@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py — BASELINE.json's metric on its config: queries/sec, 10M-doc Zipfian corpus, 3-term AND,
-BM25 top-100 (config C2), at 1/2/4/8 B200.
+BM25 top-100 (config C2), at 1/2/4/8 H100.
 
     python bench.py --gpus N --steps K --warmup W            our CUDA path (torchrun for N>1)
     python bench.py --impl reference --gpus N --steps K ...  the reference's own CPU Enquire::get_mset
@@ -14,6 +14,10 @@ A "step" is one pass of the hot path over one batch of BATCH synthetic queries.
   roofline — decode+intersect+score kernel: algorithmic bytes (SURVEY.md §8d) / its CUDA-event time.
   cpu_baseline — the compiled reference (oracle/_ref) on the box's host cores, rank 0, N=1 only.
   parity — N=1: the (docid, weight) dump of the compiled reference on the SAME 10M-doc corpus against the CUDA MSets.
+--dump-outputs DIR writes, after the timed steps, the results of the last step of both timed regions as .npy files
+(float64; docids < 2^32 are exact): replay_* (device-resident replay, this rank's result slab) and e2e_* (the MSets
+xgm_search_wait hands its caller; N > 1: rank 0's merged slice).  Inputs are seeded, so two builds run with the same
+arguments can be compared file by file.
 N>1 is strong scaling: the same 10M-doc corpus split into N interleaved docid shards (Xapian's own
 scheme, backends/multi.h:37-70), every query runs on every shard with global statistics (exchanged per
 batch, inside the e2e region), and the per-GPU top-k are merged after one all-to-all: every rank merges
@@ -42,7 +46,7 @@ TOPRANKS = 1000
 UNIT = "queries/s"
 
 # BASELINE.json's configurations (SURVEY.md section 8d).  C2 is the one `metric` is quoted on and the default;
-# the others are run with --config and their lines kept under profiles/.
+# the others are run with --config.
 CONFIGS = {
     "C2": dict(metric="queries/sec, 10M-doc 3-term AND BM25 top-100", op="AND", nterms=3, topk=100, batch=4096,
                workload="C2: 10M docs, V=1M Zipf(1) terms, 3-term OP_AND, BM25, get_mset(0,100)",
@@ -112,7 +116,7 @@ def ref_query_line(cfg, q, check_at_least=0):
 
 
 # ---------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling
 # ---------------------------------------------------------------------------------------------
 
 class ClockSampler:
@@ -245,7 +249,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 # ---------------------------------------------------------------------------------------------
@@ -391,6 +395,49 @@ class CudaArray:
     def __init__(self, ptr: int, shape, typestr: str):
         self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (int(ptr), False),
                                          "version": 2}
+
+
+def read_slab(searcher, batch, topk):
+    """The device result slab of a searcher (weights | docids | per-query records), copied to the host."""
+    import numpy as np
+    import torch
+    base, nbytes, off_d, off_c, stride = searcher.device_slab()
+    raw = torch.as_tensor(CudaArray(base, (nbytes,), "|u1"), device="cuda").cpu().numpy()
+    rec = raw[off_c:off_c + batch * 32].view(np.uint32).reshape(batch, 8)
+    return {"weights": raw[:batch * stride * 8].view(np.float64).reshape(batch, stride)[:, :topk],
+            "docids": raw[off_d:off_d + batch * stride * 4].view(np.uint32).reshape(batch, stride)[:, :topk],
+            "n": rec[:, 0], "exact": rec[:, 1]}
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(out_dir, groups):
+    """Write <group>_<name>.npy in float64.  Entries past a query's n are zeroed (the buffers are reused between
+    batches).  Over DUMP_LIMIT bytes, a fixed seeded sample of the queries (rows) is written, the same in every run."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    for g, d in groups.items():
+        n = np.asarray(d["n"]).astype(np.int64)
+        cols = np.arange(d["weights"].shape[1])
+        for k, v in d.items():
+            v = np.asarray(v).astype(np.float64)
+            if k in ("weights", "docids"):
+                v = np.where(cols[None, :] < n[:, None], v, 0.0)
+            arrays[f"{g}_{k}"] = v
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT:
+        for g in groups:
+            rows = len(arrays[f"{g}_n"])
+            keep = max(1, int(rows * DUMP_LIMIT / total))
+            idx = np.sort(np.random.default_rng(SEED).choice(rows, keep, replace=False))
+            for k in list(arrays):
+                if k.startswith(g + "_"):
+                    arrays[k] = arrays[k][idx]
+            arrays[f"{g}_rows"] = idx.astype(np.float64)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), a)
 
 
 def ours(args):
@@ -606,6 +653,8 @@ def ours(args):
     barrier()
     sampler.end()
     dev_ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        replay_out = read_slab(searchers[(args.steps - 1) % 2 if world > 1 else 0], BATCH, TOPK)
     # per-launch time of the dominant kernel: K more replays, reading each launch's own events
     for k in range(args.steps):
         searchers[0].replay()
@@ -657,7 +706,7 @@ def ours(args):
         for j in range(max(0, args.steps - LAG), args.steps):
             finish(j)
     for j in range(max(0, args.steps - NSEARCH), args.steps):
-        wait(searchers[j % NSEARCH])
+        last = wait(searchers[j % NSEARCH])  # N = 1: the host buffers holding batch j's MSets
     pending = (args.steps - 1) % NSEARCH
     torch.cuda.synchronize()
     t1 = time.perf_counter()
@@ -673,6 +722,17 @@ def ours(args):
         d2h += QL * TOPK * 12 + QL * 4
     clocks = sampler.stop()
     e2e_value = BATCH * args.steps / e2e_s
+    if args.dump_outputs and rank == 0:
+        if world > 1:
+            hw, hd, hn = host_out[pending]
+            e2e_out = {"weights": hw.numpy().reshape(QL, TOPK), "docids": hd.numpy().reshape(QL, TOPK), "n": hn.numpy()}
+        else:
+            d, w, _, inf = last
+            e2e_out = {"weights": w.reshape(-1, TOPK)[:BATCH], "docids": d.reshape(-1, TOPK)[:BATCH],
+                       "n": np.array([inf[i].n for i in range(BATCH)]),
+                       "bounds": np.array([(inf[i].matches_lower_bound, inf[i].matches_estimated, inf[i].matches_upper_bound)
+                                           for i in range(BATCH)])}
+        dump_outputs(args.dump_outputs, {"replay": replay_out, "e2e": e2e_out})
 
     # ---- p50 latency at batch = 1 through the C-ABI (rank-local) ----
     lat = []
@@ -694,19 +754,6 @@ def ours(args):
     achieved = alg_bytes / 1e9 / (kern_ms / 1e3)
     launches_per_step = int(st0.kernel_launches) + (4 if world > 1 else 0)
 
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", f"r2_{cfg['name'].lower()}_match_kernel.json")
-    if os.path.exists(tp) and world == 1:
-        try:
-            prof = json.load(open(tp))
-            # the capture is only a cross-reference while the kernel source is the one it was taken from
-            import hashlib
-            src = open(os.path.join(ROOT, "xapiand_b200", "csrc", "xgm_kernels.cu"), "rb").read()
-            if prof.get("queries_per_launch") == BATCH and prof.get("kernels_sha16") == hashlib.sha256(src).hexdigest()[:16]:
-                traffic = prof["dram_bytes_read"] + prof["dram_bytes_write"]
-                traffic_src = f"profiles/{os.path.basename(tp)} (ncu dram__bytes_read+write of one launch, same kernel source hash)"
-        except Exception:
-            pass
     step_parts = {"match_kernel_ms": kern_ms, "topk_kernel_ms": statistics.mean(topk_ms), "host_plan_ms": float(bs.host_plan_ms),
                   "host_scatter_ms": float(bs.host_wait_ms)}
     if world > 1:
@@ -717,7 +764,7 @@ def ours(args):
             "scaling": "strong" if cfg["name"] != "C4" else "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": {"workload": cfg["workload"], "docs": cfg["docs"], "vocab": VOCAB, "queries_per_step": BATCH,
                        "topk": TOPK, "shards": world, "shard_docs": int(info.doccount),
-                       "cache": "inputs larger than L2: one step streams %.0f MB of posting columns (L2 = 126 MB)" % (alg_bytes / 1e6),
+                       "cache": "inputs larger than L2: one step streams %.0f MB of posting columns (L2 = 50 MB)" % (alg_bytes / 1e6),
                        "index_bytes": int(info.bytes_docids + info.bytes_wdfs + info.bytes_headers + info.bytes_doclen),
                        "index_build_s": round(build_s, 1),
                        "value_is": "device-resident replay of one planned batch (kernel throughput); e2e is the end-to-end number"},
@@ -728,8 +775,7 @@ def ours(args):
                                 ("; per batch the phase-1 statistics exchange, the all-to-all and the merge" if world > 1 else "")},
             "gpu_launches": launches_per_step * args.steps,
             "roofline": {"bound": "hbm", "kernel": cfg["kernel"],
-                         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                         "traffic_source": traffic_src,
+                         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes,
                          "kernel_ms_per_launch": kern_ms},
             "step_breakdown_ms": step_parts, "step_bound_by": bound, "host_cpus": host_cpus,
@@ -773,7 +819,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true", help="skip the dump diff against the compiled reference")
     ap.add_argument("--config", default="C2", choices=sorted(CONFIGS), help="BASELINE.json configuration (default C2)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the results of their last step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return reference_arm(args)
     return ours(args)

@@ -1,4 +1,4 @@
-/* xgm.h — C-ABI of the B200-native inverted-index matcher (libxgm.so).
+/* xgm.h — C-ABI of the H100-native inverted-index matcher (libxgm.so).
  *
  * This is the drop-in boundary for ONE path of Kronuz/Xapiand: everything from
  * Matcher::get_local_mset (src/xapian/matcher/matcher.cc:346-542) downward — PostList tree

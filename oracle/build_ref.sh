@@ -69,6 +69,11 @@ build_xgm() {
   build_mv _xgm
 }
 
+# a changed build configuration invalidates every object built under the old one
+if [ -f "$O/libxapian_ref.so" ] && { [ "$HERE/ref_config.h" -nt "$O/libxapian_ref.so" ] || [ "$HERE/ref_uuid.h" -nt "$O/libxapian_ref.so" ]; }; then
+  rm -rf "$O"
+fi
+
 if [ -f "$O/libxapian_ref.so" ] && [ "${FORCE:-0}" != "1" ]; then
   echo "build_ref: $O/libxapian_ref.so already built (FORCE=1 to rebuild)"
   build_mv ""
@@ -76,8 +81,9 @@ if [ -f "$O/libxapian_ref.so" ] && [ "${FORCE:-0}" != "1" ]; then
   exit 0
 fi
 
-mkdir -p "$O/gen/xapian/unicode" "$O/gen/xapian/languages" "$O/obj"
+mkdir -p "$O/gen/xapian/unicode" "$O/gen/xapian/languages" "$O/gen/uuid" "$O/obj"
 cp "$HERE/ref_config.h" "$O/gen/config.h"
+cp "$HERE/ref_uuid.h" "$O/gen/uuid/uuid.h"
 # generated headers, by the reference's own generators (CMakeLists.txt:402-412, 472-479)
 (cd "$O/gen" && perl -w -I "$R/xapian" "$R/xapian/generate-exceptions")
 perl "$R/xapian/unicode/gen_c_istab" "$O/gen/xapian/unicode/c_istab.h"

@@ -104,7 +104,7 @@
 #define FOLLOWS_IEEE 1
 #define SOCKLEN_T socklen_t
 #define STRERROR_R_CHAR_P 1
-#define USE_PROC_FOR_UUID 1
+#define HAVE_UUID_UUID_H 1 /* oracle/ref_uuid.h, not /proc/sys/kernel/random/uuid */
 #define XAPIAN_LIB_BUILD 1
 #define SIZEOF_SHORT 2
 #define SIZEOF_INT 4

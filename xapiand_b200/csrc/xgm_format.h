@@ -13,7 +13,7 @@
  *           only touches it for documents that survive.
  *   bitmaps[]/ranks[]  optional per-term membership bitmap (bit d = docid d has the term) plus a rank
  *           directory (postings before every 256-docid group), kept for terms frequent enough that the
- *           bitmap costs at most XGM_BITMAP_K bits per posting.  HBM is plentiful (180 GB) and the
+ *           bitmap costs at most XGM_BITMAP_K bits per posting.  HBM is plentiful (80 GB) and the
  *           leapfrog of an AND is at heart a membership test: probing a bitmap replaces decoding the
  *           longer lists entirely; the rank directory gives the posting's index, hence its wdf.
  *   doclen[] dense u32 per docid (the reference keeps a second vbyte stream under key "\0\xe0",

@@ -134,7 +134,7 @@ struct xgm_index {
     uint64_t slot_min[XGM_MAX_SLOTS] = {};
     uint32_t slot_freq[XGM_MAX_SLOTS] = {}; /* documents with a value in the slot (Database::get_value_freq) */
     bool slot_exact[XGM_MAX_SLOTS] = {};
-    int sm_count = 148;
+    int sm_count = 132; /* H100 SXM; replaced by the device's count at upload */
     /* Large batches fill the GPU on their own: the kernels of all searchers of this index go through one
      * FIFO compute stream (copies stay on the searchers' streams), so that batch k's results are not
      * delayed by batch k+1's kernels sharing the SMs with them. */

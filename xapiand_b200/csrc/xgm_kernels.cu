@@ -1,4 +1,4 @@
-/* xgm_kernels.cu — sm_100a kernels of the matcher hot path.
+/* xgm_kernels.cu — sm_90a (H100) kernels of the matcher hot path.
  *
  *   xgm_and_kernel    decode + warp-galloping intersection + fused BM25 (reference:
  *                     GlassPostList::next/skip_to glass_postlist.cc:768-991, MultiAndPostList::
@@ -1027,8 +1027,8 @@ struct __align__(16) Bm3Scratch {
     uint64_t dbar[4];
 };
 /* 4.6 KB per warp, 37 KB per CTA: with 4 CTAs per SM the shared-memory carve-out stays at 164 KB and the
- * bitmap probes keep ~90 KB of L1 (a first version with 51 KB per CTA pushed the carve-out to 228 KB and lost
- * 19 % to L1 misses of the probes). */
+ * bitmap probes keep ~90 KB of L1 (51 KB per CTA would push the carve-out to 228 KB and leave the probes
+ * almost no L1). */
 
 /* Highest bin with at least topk stored matches at or above it → raise the query's pruning bucket
  * (the warp-cooperative half of emit_matches_impl). */
@@ -3162,7 +3162,7 @@ __global__ void xgm_expand_items_kernel(const XgmWorkItem* __restrict__ seg, uin
 /* Range-major expansion (bitmap AND list, large batches).  The docid space is cut into ranges of
  * 2^range_bits documents and the work list is ordered range by range, every query's driver blocks of
  * range 0 first, then range 1, ...: at any moment all warps probe the same slice of every membership
- * bitmap (lastdocid/8 bytes per term shrink to 2^range_bits/8), which stays in the 126 MB L2 while the
+ * bitmap (lastdocid/8 bytes per term shrink to 2^range_bits/8), which stays in the 50 MB L2 while the
  * whole batch walks over it — each bitmap is read from HBM about once per batch instead of once per query
  * that uses it.  Every query still advances through the whole batch, so thresholds rise early as with the
  * level order.  Three small kernels: per (range, segment) the driver blocks whose first docid falls in
@@ -3332,7 +3332,11 @@ cudaError_t xgm_launch_topk(const XgmKernelParams& p, uint32_t nq, cudaStream_t 
 cudaError_t xgm_launch_decode(const XgmKernelParams& p, uint32_t blk_begin, uint32_t nblocks, uint32_t* out_d,
                               uint32_t* out_w, cudaStream_t s) {
     int grid = (int)((nblocks + MATCH_WARPS - 1) / MATCH_WARPS);
-    if (grid > 148 * 8) grid = 148 * 8;
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (sms < 1) sms = 132; /* H100 SXM */
+    if (grid > sms * 8) grid = sms * 8;
     if (grid < 1) grid = 1;
     xgm_decode_kernel<<<grid, MATCH_WARPS * 32, 0, s>>>(p, blk_begin, nblocks, out_d, out_w);
     return cudaGetLastError();
