@@ -259,6 +259,8 @@ typedef struct xgm_mset_info {
  * each.  xgm_search* replace Matcher::get_local_mset (src/xapian/matcher/matcher.cc:346-542, declared in
  * matcher.h:92-108) for the query shapes listed at xgm_query. */
 xgm_status xgm_searcher_new(const xgm_index*, uint32_t max_batch, uint32_t max_topk, xgm_searcher** out);
+/* May run after xgm_index_close of the searcher's index (a garbage collector frees the two in any order); the
+ * searcher must not search once its index is closed. */
 void xgm_searcher_free(xgm_searcher*);
 
 /* Asynchronous batch: plan on the host, copy the plan to the device, launch the kernels, start the

@@ -206,6 +206,19 @@ def test_background_submit_matches_synchronous(edge):
                    (m.matches_lower_bound, m.matches_estimated_raw, m.matches_upper_bound), (b, i)
 
 
+def test_searcher_freed_after_its_index():
+    """A garbage collector frees an index and a searcher on it in any order.  Freeing the searcher must not read the
+    closed index: it once took its device number from there, and the failed cudaSetDevice of a freed index surfaced
+    as the launch error of the next, unrelated batch."""
+    ix = xgm.Index.synthetic(2000, 300)
+    s = xgm.Searcher(ix, max_batch=4, max_topk=16)
+    assert s.search([xgm.Query(xgm.OP_AND, [0, 1], maxitems=5)])[0].status == 0
+    ix.close()
+    s.close()
+    ix2 = xgm.Index.synthetic(2000, 300)
+    assert xgm.Searcher(ix2, max_batch=4, max_topk=16).search([xgm.Query(xgm.OP_AND, [0, 1], maxitems=5)])[0].status == 0
+
+
 def test_process_exits_after_a_large_batch():
     """Batches of >= 512 queries are planned on the library's helper threads, which stay parked for the life of
     the process: the host program must still exit (a static pool object whose condition variable was destroyed

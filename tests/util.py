@@ -21,6 +21,22 @@ def gen_queries(rng: random.Random, n, topranks, ndocs, ops=("AND",), ks=(3,), m
     return out
 
 
+def assert_matches_oracle(got, ref, ctx=""):
+    """assert_mset_equal, except that what an approximation flag licenses is checked in its weaker form:
+    with BOUNDS_APPROX (1) lb <= ref.lb and lb <= est <= ub; with COUNT_LOWER_BOUND (2) exact <= ref.exact.
+    The upper bound is always exact."""
+    approx = bool(got.flags & 1)
+    assert_mset_equal(got, ref, ctx, check_counts=not approx)
+    assert got.matches_upper_bound == ref.ub, f"{ctx}: ub {got.matches_upper_bound} vs {ref.ub}"
+    if got.flags & 2:
+        assert got.exact_matches <= ref.exact, f"{ctx}: exact {got.exact_matches} > {ref.exact}"
+    else:
+        assert got.exact_matches == ref.exact, f"{ctx}: exact {got.exact_matches} vs {ref.exact}"
+    if approx:
+        assert got.matches_lower_bound <= ref.lb, f"{ctx}: lb {got.matches_lower_bound} > {ref.lb}"
+        assert got.matches_lower_bound <= got.matches_estimated_raw <= got.matches_upper_bound, f"{ctx}: lb/est/ub"
+
+
 def assert_mset_equal(got, ref, ctx="", check_counts=True):
     """got: xgm.MSet, ref: oracle MSet. docids in order, weights bit-exact."""
     assert got.status == 0, f"{ctx}: status {got.status}"

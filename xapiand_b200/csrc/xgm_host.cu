@@ -918,6 +918,7 @@ struct PlannedQuery {
 
 struct xgm_searcher {
     const xgm_index* ix = nullptr;
+    int device = 0; /* ix->device, kept so that freeing the searcher never reads an index already closed */
     uint32_t max_batch = 0, max_topk = 0, match_cap = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
@@ -1031,7 +1032,7 @@ extern "C" void xgm_searcher_free(xgm_searcher* s) {
         s->cv.notify_all();
         s->worker.join();
     }
-    cudaSetDevice(s->ix->device);
+    cudaSetDevice(s->device);
     if (s->stream) cudaStreamSynchronize(s->stream);
     cudaFreeHost(s->h_queries); cudaFreeHost(s->h_items); cudaFreeHost(s->h_items_or); cudaFreeHost(s->h_items_bm); cudaFreeHost(s->h_out_w); cudaFreeHost(s->h_out_d);
     cudaFreeHost(s->h_out_k); cudaFreeHost(s->h_info); cudaFreeHost(s->h_raise); cudaFree(s->d_raise); cudaFreeHost(s->h_qstate); cudaFreeHost(s->h_tileq); cudaFree(s->d_tileq);
@@ -1099,7 +1100,7 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
     if (max_batch >= (1u << 25)) return fail(XGM_E_INVALID, "max_batch %u too large", max_batch);
     CUDA_TRY(cudaSetDevice(ix->device));
     std::unique_ptr<xgm_searcher, void (*)(xgm_searcher*)> s(new xgm_searcher(), xgm_searcher_free);
-    s->ix = ix; s->max_batch = max_batch; s->max_topk = max_topk;
+    s->ix = ix; s->device = ix->device; s->max_batch = max_batch; s->max_topk = max_topk;
     /* candidates a query may buffer before its pruning threshold settles (~k(1+ln(M/k)) arrive above
      * a rising threshold) and how many of them the top-k kernel can hold in shared memory */
     s->match_cap = std::min<uint32_t>(65536, std::max<uint32_t>(8192, 32 * max_topk));
