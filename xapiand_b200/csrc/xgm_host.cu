@@ -961,7 +961,7 @@ struct xgm_searcher {
     uint32_t* d_rng_total = nullptr;
     uint32_t* h_rng_total = nullptr;
     bool range_mode = false;
-    uint32_t range_bits = 18, nranges = 1;
+    uint32_t range_bits = 17, nranges = 1; /* XGM_RANGE_BITS: 2^17 docids per range (DESIGN.md §3.1) */
     struct OrGroup { uint32_t seg_off, nseg, level_off, nlevels, out_off, total; };
     std::vector<OrGroup> or_groups; /* OR list: one level-ordered expansion per leaf position */
     uint32_t* d_topk_list = nullptr; /* [max_batch] queries left to the CTA-per-query top-k kernel */

@@ -1018,7 +1018,7 @@ __global__ void __launch_bounds__(BM_WARPS * 32, 4) xgm_and_bm_kernel(XgmKernelP
 #define BM3_Q2CAP 64
 
 struct __align__(16) Bm3Scratch {
-    uint32_t dstage[4][STAGE_WORDS];
+    uint32_t dstage[4][STAGE_WORDS]; /* packed driver blocks (bulk copies), then their decoded docids */
     uint32_t q1did[BM3_Q1CAP]; /* stage 1 belongs to the current work item (one query) */
     uint16_t q1src[BM3_Q1CAP]; /* (driver block - b0) << 7 | position */
     uint32_t q2did[BM3_Q2CAP]; /* stage 2 lives as long as the warp: entries carry their query */
@@ -1260,6 +1260,19 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
             } else {
                 c[4] = c[5] = c[6] = c[7] = 0u;
             }
+            /* Interleave the postings across the lanes, through the staging buffers they were decoded from: after
+             * this, slot k of lane l holds posting 32 (k & 3) + l of block k >> 2.  decode_docids leaves a lane
+             * postings 4l..4l+3, at C2's driver density ~85 bytes of bitmap from its neighbour's, so each probe load
+             * below would touch ~21 cache lines per warp; interleaved, its 32 lanes are 32 consecutive postings.  (An
+             * absent second block transposes its zeros.)  The bulk-copy engine refills these buffers for a later
+             * pair: the proxy fence orders this generic-proxy write before that async-proxy one. */
+            __syncwarp();
+            reinterpret_cast<uint4*>(ws.dstage[cur])[lane] = make_uint4(c[0], c[1], c[2], c[3]);
+            reinterpret_cast<uint4*>(ws.dstage[cur + 1])[lane] = make_uint4(c[4], c[5], c[6], c[7]);
+            __syncwarp();
+#pragma unroll
+            for (int k = 0; k < 8; ++k) c[k] = ws.dstage[cur + (k >> 2)][32 * (k & 3) + lane];
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             /* the skip_to/check of the leapfrog: one bitmap word per candidate, all loads issued together */
             uint32_t w[8];
             if (cnt0 + cnt1 == 2u * XGM_BLOCK) { /* two full blocks (warp-uniform): no per-posting predicates */
@@ -1267,7 +1280,9 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
 #pragma unroll
                 for (int k = 0; k < 8; ++k) w[k] = __ldg(bm1 + (c[k] >> 5));
             } else {
-                const int m0 = min(4, max(0, (int)cnt0 - 4 * (int)lane)), m1 = min(4, max(0, (int)cnt1 - 4 * (int)lane));
+                /* slot k < 4 holds posting 32k + lane of the first block: the lane has (cnt + 31 - lane) / 32 of
+                 * each block's cnt postings (cnt <= 128, and 0 of an absent second block) */
+                const uint32_t m0 = (cnt0 + 31u - lane) >> 5, m1 = (cnt1 + 31u - lane) >> 5;
                 alive = ((1u << m0) - 1u) | (((1u << m1) - 1u) << 4);
 #pragma unroll
                 for (int k = 0; k < 8; ++k) w[k] = (alive >> k & 1u) ? __ldg(bm1 + (c[k] >> 5)) : 0u;
@@ -1287,12 +1302,12 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
                 if (surv) {
                     const uint32_t lt = (1u << lane) - 1u;
                     uint32_t slot = qn1 + __popc(B & lt) + __popc(B0 & lt) + 2u * __popc(B1 & lt) + 4u * __popc(B2 & lt);
-                    const uint32_t rb = (db - it_b0) << 7 | 4 * lane;
+                    const uint32_t rb = (db - it_b0) << 7 | lane;
 #pragma unroll
                     for (int k = 0; k < 8; ++k)
                         if (surv >> k & 1u) {
                             ws.q1did[slot] = c[k];
-                            ws.q1src[slot] = (uint16_t)(rb + ((k >> 2) << 7) + (k & 3));
+                            ws.q1src[slot] = (uint16_t)(rb + ((k >> 2) << 7) + ((k & 3) << 5));
                             ++slot;
                         }
                 }
