@@ -1112,6 +1112,49 @@ __device__ __forceinline__ void emit_match_lanes(const XgmKernelParams& p, uint3
     }
 }
 
+/* Next non-empty group of the grouped bitmap AND list (work_counter[6] counts them), packed as end << 32 | first
+ * item; 0: none left. */
+__device__ __noinline__ unsigned long long bm3_fetch_group(const XgmKernelParams& p, uint32_t nitems_bm) {
+    for (;;) {
+        const uint32_t g = atomicAdd(p.work_counter + 6, 1u);
+        if (g >= p.ngroups) return 0ull;
+        const uint32_t a = __ldg(p.grp_off + g), b = g + 1 < p.ngroups ? __ldg(p.grp_off + g + 1) : nitems_bm;
+        if (a < b) return (unsigned long long)b << 32 | a;
+    }
+}
+
+/* Next item of the grouped bitmap AND list for the calling lane's warp (one lane per warp; nitems_bm: no work
+ * left).  cur holds the CTA's current group, items [low word, high word), and next the group after it (~0 while
+ * it is being fetched).  No warp waits for another to finish its item: the warp whose claim equals the end
+ * installs the next group and fetches the one after; the others spin for the short time that takes.  Kept out of
+ * line so that the pair step keeps its registers. */
+__device__ __noinline__ uint32_t bm3_claim_grouped(const XgmKernelParams& p, uint32_t nitems_bm, unsigned long long* cur,
+                                                   unsigned long long* next) {
+    volatile unsigned long long* vcur = cur;
+    volatile unsigned long long* vnext = next;
+    for (;;) {
+        const unsigned long long cw = atomicAdd(cur, 1ull);
+        const uint32_t nx = (uint32_t)cw, en = (uint32_t)(cw >> 32);
+        if (nx < en) return nx;
+        if (nx == en) {
+            unsigned long long n;
+            while ((n = *vnext) == ~0ull) __nanosleep(32); /* the previous installer is still fetching */
+            if (n == 0ull) return nitems_bm; /* cur stays used up: every later claim ends here too */
+            *vnext = ~0ull; /* not to be installed twice */
+            __threadfence_block();
+            *vcur = n + 1u; /* this warp takes the group's first item */
+            *vnext = bm3_fetch_group(p, nitems_bm);
+            return (uint32_t)n;
+        }
+        for (;;) {
+            const unsigned long long v = *vcur;
+            if ((uint32_t)v < (uint32_t)(v >> 32)) break;
+            if (*vnext == 0ull) return nitems_bm;
+            __nanosleep(32);
+        }
+    }
+}
+
 /* One flat loop with four states, so that each piece of code exists once and nothing is called from the hot
  * path: score 32 matches (stage 2 full, or out of work) → finish 32 candidates (stage 1 full, or the item
  * ended) → fetch the next work item → decode and probe the next pair of driver blocks. */
@@ -1121,7 +1164,13 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
     Bm3Scratch* scratch = reinterpret_cast<Bm3Scratch*>(bm3_raw);
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     Bm3Scratch& ws = scratch[warp];
+    /* grouped list (p.ngroups != 0): the CTA's current group and the next one (bm3_claim_grouped) */
+    __shared__ unsigned long long grp_cur, grp_next;
     if (lane < 4) mbar_init(&ws.dbar[lane], 1);
+    if (threadIdx.x == 0) {
+        grp_cur = 0;
+        if (p.ngroups != 0) grp_next = bm3_fetch_group(p, p.nitems_bm_dev ? __ldg(p.nitems_bm_dev) : p.nitems_bm);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
     uint32_t phases = 0;
@@ -1224,7 +1273,12 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
         /* ---- next work item ---- */
         if (item_end) {
             uint32_t item = 0;
-            if (lane == 0) item = atomicAdd(p.work_counter + 6 + p.pass, 1u);
+            if (p.ngroups == 0) {
+                if (lane == 0) item = atomicAdd(p.work_counter + 6 + p.pass, 1u);
+            } else if (lane == 0) {
+                /* the queries of a group probe the same bitmap in the same docid range: the CTA's warps share L1 lines */
+                item = bm3_claim_grouped(p, nitems_bm, &grp_cur, &grp_next);
+            }
             item = __shfl_sync(FULL, item, 0);
             if (item >= nitems_bm) { done = true; continue; }
             const XgmWorkItem wi = p.items_bm[item];
@@ -3263,16 +3317,20 @@ __global__ void __launch_bounds__(XGM_SCAN_THREADS) xgm_range_scan_kernel(uint32
 
 __global__ void __launch_bounds__(XGM_RNG_THREADS) xgm_range_fill_kernel(
     const XgmWorkItem* __restrict__ seg, uint32_t nseg, uint32_t nranges, uint32_t bpi, const uint32_t* __restrict__ lo_in,
-    const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ block_off, XgmWorkItem* __restrict__ out) {
+    const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ block_off, XgmWorkItem* __restrict__ out,
+    uint32_t nruns, uint32_t* __restrict__ grp_off) {
     __shared__ uint32_t warp_sums[XGM_RNG_THREADS / 32];
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     const bool in = t < nranges * nseg;
     const uint32_t n = in ? cnt[t] : 0u;
     uint32_t total;
     const uint32_t off = block_off[blockIdx.x] + block_exclusive_scan_256(n, warp_sums, &total);
-    if (n == 0) return;
+    if (!in) return;
     const uint32_t j = t / nseg, sidx = t - j * nseg;
     const XgmWorkItem sg = seg[sidx];
+    /* the first segment of run r (pad = 0x80000000 | r) starts group (j, r) */
+    if (grp_off != nullptr && (sg.pad >> 31) != 0) grp_off[j * nruns + (sg.pad & 0x7fffffffu)] = off;
+    if (n == 0) return;
     const uint32_t lo = lo_in[t];
     const uint32_t hi = j + 1 == nranges ? sg.b0 : lo_in[t + nseg];
     XgmWorkItem w;
@@ -3287,13 +3345,14 @@ __global__ void __launch_bounds__(XGM_RNG_THREADS) xgm_range_fill_kernel(
 
 cudaError_t xgm_launch_expand_ranges(const XgmWorkItem* seg, uint32_t nseg, const XgmDevQuery* queries, const XgmBlockHdr* hdr,
                                      uint32_t nranges, uint32_t range_bits, uint32_t bpi, uint32_t* lo, uint32_t* cnt,
-                                     uint32_t* off, uint32_t* total, XgmWorkItem* out, cudaStream_t s) {
+                                     uint32_t* off, uint32_t* total, XgmWorkItem* out, uint32_t nruns, uint32_t* grp_off,
+                                     cudaStream_t s) {
     const uint32_t n = nranges * nseg;
     if (n == 0) return cudaSuccess;
     const uint32_t nb = (n + XGM_RNG_THREADS - 1) / XGM_RNG_THREADS; /* `off` holds the nb block sums / offsets */
     xgm_range_count_kernel<<<nb, XGM_RNG_THREADS, 0, s>>>(seg, nseg, queries, hdr, nranges, range_bits, bpi, lo, cnt, off);
     xgm_range_scan_kernel<<<1, XGM_SCAN_THREADS, 0, s>>>(off, nb, total);
-    xgm_range_fill_kernel<<<nb, XGM_RNG_THREADS, 0, s>>>(seg, nseg, nranges, bpi, lo, cnt, off, out);
+    xgm_range_fill_kernel<<<nb, XGM_RNG_THREADS, 0, s>>>(seg, nseg, nranges, bpi, lo, cnt, off, out, nruns, grp_off);
     return cudaGetLastError();
 }
 
