@@ -41,11 +41,10 @@ struct XgmKernelParams {
     const XgmWorkItem* items_bm;  /* bitmap AND kernel work list */
     uint32_t nitems, nitems_or, nitems_bm;
     const uint32_t* nitems_bm_dev; /* non-null: item count of the bitmap AND list lives on the device (range-major expansion) */
-    /* range-major bitmap AND list cut into groups: range j, run r of queries that probe the same list (terms[1]).
-     * Group g = j * nruns + r holds items [grp_off[g], grp_off[g + 1]) (the last one ends at the item count).
-     * ngroups = 0: no groups, the warps take items one by one from the work counter. */
-    const uint32_t* grp_off;
-    uint32_t ngroups, nruns;
+    /* range-major bitmap AND list: its segments, sorted by driver list.  An item serves the run of queries
+     * bm_segs[query .. query + pad).query, which share the driver.  Null (level order): the item's query field is
+     * its one query. */
+    const XgmWorkItem* bm_segs;
     uint32_t nq;
     uint32_t* work_counter;       /* [10],[11] OR items of xgm_or3_kernel (first / second pass); [12],[13] tiles of xgm_or_tile_kernel; [14],[15] items of xgm_or3_kernel<PHASE 1>; [8..9] 64-bit pool reservation; [0] AND items, [1] OR items, [2],[3] same for the second pass, [4] #queries to re-run, [5] overflow-pool entries reserved, [6],[7] bitmap-AND items (first / second pass) */
     uint32_t pass;                /* 0 = first pass, 1 = re-run of overflowed queries with their exact b* */
@@ -85,10 +84,9 @@ cudaError_t xgm_launch_and_bm(const XgmKernelParams& p, int grid, cudaStream_t s
 int xgm_and_bm_occupancy_blocks_per_sm();
 cudaError_t xgm_launch_expand(const XgmWorkItem* seg, uint32_t nseg, uint32_t total, const uint32_t* level_start,
                               uint32_t nlevels, uint32_t bpi, XgmWorkItem* out, cudaStream_t s);
-cudaError_t xgm_launch_expand_ranges(const XgmWorkItem* seg, uint32_t nseg, const XgmDevQuery* queries, const XgmBlockHdr* hdr,
-                                     uint32_t nranges, uint32_t range_bits, uint32_t bpi, uint32_t* lo, uint32_t* cnt,
-                                     uint32_t* off, uint32_t* total, XgmWorkItem* out, uint32_t nruns, uint32_t* grp_off,
-                                     cudaStream_t s);
+cudaError_t xgm_launch_expand_ranges(const XgmWorkItem* runs, uint32_t nruns, const XgmBlockHdr* hdr, uint32_t nranges,
+                                     uint32_t range_bits, uint32_t bpi, uint32_t* lo, uint32_t* cnt, uint32_t* off,
+                                     uint32_t* total, XgmWorkItem* out, cudaStream_t s);
 cudaError_t xgm_launch_or(const XgmKernelParams& p, int grid, cudaStream_t s);
 int xgm_or_occupancy_blocks_per_sm();
 cudaError_t xgm_launch_or3(const XgmKernelParams& p, int grid, int phase, cudaStream_t s);

@@ -83,6 +83,12 @@ struct XgmWorkItem {
     uint32_t pad;
 };
 
+/* Range-major bitmap AND list: at most this many queries with the same driver list share one work item (a run),
+ * which decodes the driver's blocks once for all of them.  Longer runs decode less but make fewer, longer items per
+ * docid range, so more ranges are in flight at once and their bitmap slices outgrow L2 (DESIGN.md §6).  The AND
+ * kernel tags a queued candidate with its query's slot in the run in 4 bits: at most 16. */
+#define XGM_BM_RUN 3
+
 /* per-query running state of a batch (zeroed before every launch) */
 struct XgmQState {
     uint32_t total;            /* documents matching the boolean structure */

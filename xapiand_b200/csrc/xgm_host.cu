@@ -962,7 +962,7 @@ struct xgm_searcher {
     uint32_t* h_rng_total = nullptr;
     bool range_mode = false;
     uint32_t range_bits = 17, nranges = 1; /* XGM_RANGE_BITS: 2^17 docids per range (DESIGN.md §3.1) */
-    uint32_t nruns = 0, ngroups = 0;       /* runs of segments with one probe list; groups = nranges * nruns */
+    uint32_t nruns = 0;                    /* runs of segments with one driver list (uploaded after the segments) */
     struct OrGroup { uint32_t seg_off, nseg, level_off, nlevels, out_off, total; };
     std::vector<OrGroup> or_groups; /* OR list: one level-ordered expansion per leaf position */
     uint32_t* d_topk_list = nullptr; /* [max_batch] queries left to the CTA-per-query top-k kernel */
@@ -1722,10 +1722,9 @@ static xgm_status launch_batch(xgm_searcher* s) {
                     s->stats.kernel_launches++;
                 }
             } else if (w == 2 && s->range_mode) {
-                const size_t n = (size_t)s->nranges * s->nseg[2];
-                CUDA_TRY(xgm_launch_expand_ranges(segs[2], s->nseg[2], s->d_queries, p.hdr, s->nranges, s->range_bits, s->bpi,
-                                                  s->d_rng, s->d_rng + n, s->d_rng + 2 * n, s->d_rng_total, s->d_exp[2],
-                                                  s->nruns, s->d_rng + 3 * n, cs));
+                const size_t n = (size_t)s->nranges * s->nruns;
+                CUDA_TRY(xgm_launch_expand_ranges(segs[2] + s->nseg[2], s->nruns, p.hdr, s->nranges, s->range_bits, s->bpi,
+                                                  s->d_rng, s->d_rng + n, s->d_rng + 2 * n, s->d_rng_total, s->d_exp[2], cs));
                 s->stats.kernel_launches += 3;
             } else {
                 CUDA_TRY(xgm_launch_expand(segs[w], s->nseg[w], totals[w], s->d_levels[w], s->nlevels[w], s->bpi, s->d_exp[w], cs));
@@ -1752,7 +1751,6 @@ static xgm_status launch_batch(xgm_searcher* s) {
     /* second pass: only queries whose candidate buffer overflowed do any work (device-side flag) */
     XgmKernelParams p2 = p;
     p2.pass = 1;
-    p2.ngroups = 0; /* the few re-run queries take their items one by one */
     if (s->nitems_bm) { CUDA_TRY(xgm_launch_and_bm(p2, s->grid_bm, cs)); s->stats.kernel_launches++; }
     if (s->nitems) { CUDA_TRY(launch_and(p2)); s->stats.kernel_launches++; }
     if (s->nitems_or && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p2, s->grid_or3, 0, cs)); s->stats.kernel_launches++; }
@@ -1836,38 +1834,44 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
         uint32_t* totals[3] = {&s->nitems, &s->nitems_or, &s->nitems_bm};
         for (int w = 0; w < 3; ++w) {
             std::vector<XgmWorkItem>& v = *lists[w];
-            st = ensure_items(s, v.size(), w);
+            st = ensure_items(s, w == 2 ? 2 * v.size() : v.size(), w); /* the bitmap list may add its runs */
             if (st != XGM_OK) return st;
             uint64_t run = 0;
             XgmWorkItem* h = *hbuf[w];
             s->nlevels[w] = 0;
-            if (w == 2) { s->range_mode = false; s->nruns = s->ngroups = 0; }
+            if (w == 2) { s->range_mode = false; s->nruns = 0; }
             if (w == 2 && !v.empty() && nq >= 256 && s->range_bits != 0) {
                 /* range-major order, expanded on the device (xgm_range_*_kernel): the host only bounds the
-                 * number of items — every range can add one partial item per segment */
+                 * number of items — every range can add one partial item per run */
                 s->range_mode = true;
                 s->nranges = (s->ix->lastdocid >> s->range_bits) + 1;
-                /* segments sorted by probe list (terms[1]), so that the queries of a range that probe the same bitmap
-                 * form one group, which the AND kernel hands to the warps of one CTA: they then read the same bitmap
-                 * words, through the same L1.  The first segment of run r carries 0x80000000 | r in pad
-                 * (xgm_range_fill_kernel records where each group starts).  A list with value-range predicates keeps
-                 * query order and takes items one by one: grouped, the C5 configuration (2-term AND, value range, sort
-                 * by value) measured 6 % slower, for a reason not found yet (DESIGN.md §6). */
+                /* Segments sorted by driver list (terms[0]), ties by query index.  Up to XGM_BM_RUN consecutive segments
+                 * with the same driver form a run, and the run's items serve all of its queries: the AND kernel decodes
+                 * the driver's blocks once per range and probes them for each query.  The runs follow the segments in
+                 * the upload as {first segment, #driver blocks, the driver's first header, #queries}. */
                 const XgmDevQuery* hq = s->h_queries;
-                bool group = true;
-                for (const XgmWorkItem& a : v) group = group && hq[a.query].filter == XGM_FILTER_NONE;
-                auto probe = [hq](const XgmWorkItem& a) { return hq[a.query].terms[1].bm_off; };
-                if (group) {
-                    std::sort(v.begin(), v.end(), [&](const XgmWorkItem& a, const XgmWorkItem& b) {
-                        return probe(a) != probe(b) ? probe(a) < probe(b) : a.query < b.query;
-                    });
-                    for (size_t i = 0; i < v.size(); ++i)
-                        v[i].pad = i == 0 || probe(v[i]) != probe(v[i - 1]) ? 0x80000000u | s->nruns++ : 0u;
+                auto drv = [hq](const XgmWorkItem& a) { return hq[a.query].terms[0].blk_begin; };
+                std::sort(v.begin(), v.end(), [&](const XgmWorkItem& a, const XgmWorkItem& b) {
+                    return drv(a) != drv(b) ? drv(a) < drv(b) : a.query < b.query;
+                });
+                const size_t nseg = v.size();
+                for (size_t i = 0; i < nseg; ++i) {
+                    h[i] = v[i];
+                    XgmWorkItem* last = h + nseg + s->nruns - 1;
+                    if (s->nruns != 0 && last->b1 == drv(v[i]) && last->pad < XGM_BM_RUN) {
+                        ++last->pad;
+                        continue;
+                    }
+                    h[nseg + s->nruns++] = XgmWorkItem{(uint32_t)i, v[i].b0, drv(v[i]), 1u};
+                    run += (v[i].b0 + bpi - 1) / bpi;
                 }
-                s->ngroups = s->nranges * s->nruns;
-                for (size_t i = 0; i < v.size(); ++i) { h[i] = v[i]; run += (v[i].b0 + bpi - 1) / bpi; }
-                run += (uint64_t)v.size() * s->nranges;
-                const size_t need = (size_t)s->nranges * v.size() * 4; /* first blocks, counts, offsets, groups */
+                /* most work first within each range (queries x driver blocks), so that the batch does not end on a
+                 * long item */
+                std::stable_sort(h + nseg, h + nseg + s->nruns, [](const XgmWorkItem& a, const XgmWorkItem& b) {
+                    return (uint64_t)a.pad * a.b0 > (uint64_t)b.pad * b.b0;
+                });
+                run += (uint64_t)s->nruns * s->nranges; /* every range can add one partial item per run */
+                const size_t need = (size_t)s->nranges * s->nruns * 3; /* first blocks, counts, offsets */
                 if (need > s->rng_cap) {
                     CUDA_TRY(cudaStreamSynchronize(s->stream));
                     if (s->ix->compute_stream) CUDA_TRY(cudaStreamSynchronize(s->ix->compute_stream));
@@ -1944,7 +1948,7 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     s->stats = xgm_batch_stats{};
     s->stats.algorithmic_bytes = alg;
     s->stats.work_items = s->nitems + s->nitems_or + s->nitems_bm;
-    s->stats.h2d_bytes = (uint64_t)nq * sizeof(XgmDevQuery) + (uint64_t)(s->nseg[0] + s->nseg[1] + s->nseg[2]) * sizeof(XgmWorkItem);
+    s->stats.h2d_bytes = (uint64_t)nq * sizeof(XgmDevQuery) + (uint64_t)(s->nseg[0] + s->nseg[1] + s->nseg[2] + s->nruns) * sizeof(XgmWorkItem);
     s->stats.d2h_bytes = (uint64_t)nq * sizeof(XgmDevResult) + (uint64_t)nq * s->max_topk * (8 + 4 + (s->any_sort ? 8 : 0));
     XgmKernelParams& p = s->params;
     fill_index_params(s->ix, p);
@@ -1952,8 +1956,7 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     p.items_or = s->d_exp[1]; p.nitems_or = s->nitems_or;
     p.items_bm = s->d_exp[2]; p.nitems_bm = s->nitems_bm;
     p.nitems_bm_dev = s->range_mode ? s->d_rng_total : nullptr;
-    p.ngroups = s->ngroups; p.nruns = s->nruns;
-    p.grp_off = s->ngroups ? s->d_rng + 3 * (size_t)s->nranges * s->nseg[2] : nullptr;
+    p.bm_segs = s->range_mode ? s->d_items_bm : nullptr;
     p.work_counter = reinterpret_cast<uint32_t*>(s->d_ctrl);
     p.qstate = reinterpret_cast<XgmQState*>(s->d_ctrl + XGM_CTRL_HDR);
     p.hist = reinterpret_cast<uint32_t*>(s->d_ctrl + XGM_CTRL_HDR + (size_t)s->max_batch * sizeof(XgmQState));
@@ -1981,7 +1984,8 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     if (s->nseg[1])
         CUDA_TRY(cudaMemcpyAsync(s->d_items_or, s->h_items_or, (size_t)s->nseg[1] * sizeof(XgmWorkItem), cudaMemcpyHostToDevice, s->stream));
     if (s->nseg[2])
-        CUDA_TRY(cudaMemcpyAsync(s->d_items_bm, s->h_items_bm, (size_t)s->nseg[2] * sizeof(XgmWorkItem), cudaMemcpyHostToDevice, s->stream));
+        CUDA_TRY(cudaMemcpyAsync(s->d_items_bm, s->h_items_bm, (size_t)(s->nseg[2] + s->nruns) * sizeof(XgmWorkItem),
+                                 cudaMemcpyHostToDevice, s->stream));
     for (int w = 0; w < 3; ++w)
         if (s->nlevels[w])
             CUDA_TRY(cudaMemcpyAsync(s->d_levels[w], s->h_levels[w], ((size_t)s->nlevels[w] + 1) * 4, cudaMemcpyHostToDevice, s->stream));

@@ -835,177 +835,11 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(XgmKernelP
 
 /* AND of a driver list with lists that all have membership bitmaps — the common case once HBM is used
  * for bitmaps of the frequent terms.  Warp-autonomous like xgm_and_kernel, but stripped to the fast
- * path so that more warps fit an SM (the kernel is bound by DRAM latency of the bitmap probes): per
- * iteration a warp decodes TWO driver blocks (bulk copies of the next pair already in flight), issues
- * the 8 bitmap word loads of every lane together, queues the candidates confirmed by the second list
- * and finishes them 32 at a time, one per lane (remaining bitmaps, rank → wdf, doc length, BM25 in
- * MultiAndPostList order, emission). */
-#define BM_WARPS 8
-#define BM_QCAP 288
-
-struct __align__(16) BmScratch {
-    uint32_t dstage[4][STAGE_WORDS];
-    uint32_t qdid[BM_QCAP];
-    uint32_t qsrc[BM_QCAP];
-    uint64_t dbar[4];
-};
-
-__global__ void __launch_bounds__(BM_WARPS * 32, 4) xgm_and_bm_kernel(XgmKernelParams p) {
-    __shared__ BmScratch scratch[BM_WARPS];
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    BmScratch& ws = scratch[warp];
-    if (lane < 4) mbar_init(&ws.dbar[lane], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncthreads();
-    uint32_t phases = 0;
-    const XgmBlockHdr* __restrict__ hdr = p.hdr;
-    const uint32_t stage_base = smem_u32(ws.dstage[0]);
-#define bar_base (stage_base + (uint32_t)offsetof(BmScratch, dbar))
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + 4) == 0) return;
-    /* range-major expansion counts its items on the device */
-    const uint32_t nitems_bm = p.nitems_bm_dev ? __ldg(p.nitems_bm_dev) : p.nitems_bm;
-
-    for (;;) {
-        uint32_t item = 0;
-        if (lane == 0) item = atomicAdd(p.work_counter + 6 + p.pass, 1u);
-        item = __shfl_sync(FULL, item, 0);
-        if (item >= nitems_bm) break;
-        const XgmWorkItem wi = p.items_bm[item];
-        if (p.pass != 0 && p.qstate[wi.query].rerun == 0) continue;
-        const XgmDevQuery* q = &p.queries[wi.query];
-        const uint32_t nterms = q->nterms, nall = nterms + q->nnot;
-        const uint32_t drv_begin = q->terms[0].blk_begin;
-        const uint32_t* __restrict__ bm1 = p.bitmaps + q->terms[1].bm_off;
-        uint32_t qn = 0;
-
-        auto flush = [&](uint32_t from, uint32_t count) {
-            uint32_t alive = lane < count ? 1u : 0u;
-            const uint32_t d = alive ? ws.qdid[from + lane] : 0u;
-            const uint32_t src = alive ? ws.qsrc[from + lane] : 0u;
-            for (uint32_t j = 2; j < nall && __any_sync(FULL, alive); ++j) {
-                if (alive) {
-                    const uint32_t w = __ldg(p.bitmaps + q->terms[j].bm_off + (d >> 5));
-                    /* required lists must hold the docid, the right side of an OP_AND_NOT must not */
-                    if (((w >> (d & 31)) & 1u) == (j < nterms ? 0u : 1u)) alive = 0u;
-                }
-            }
-            if (alive && q->filter && !doc_passes_filter(p, q, d)) alive = 0u;
-            double acc[4] = {0.0, 0.0, 0.0, 0.0};
-            uint32_t opt = 0;
-            if (alive) {
-                const uint32_t dlen = __ldg(&p.doclen[d]);
-                const XgmBlockHdr h0 = hdr[drv_begin + wi.b0 + (src >> 7)];
-                acc[0] = bm25_sumpart(q->terms[0].termweight, q,
-                                      unpack_gl(p.tfs, h0.tf_off, src & 127u, XGM_HDR_TF_BITS(h0.meta)), dlen);
-                for (uint32_t j = 1; j < nterms; ++j) {
-                    const uint32_t r = bitmap_rank(p, q->terms[j], d);
-                    const XgmBlockHdr bh = hdr[q->terms[j].blk_begin + (r >> 7)];
-                    const uint32_t tfj = unpack_gl(p.tfs, bh.tf_off, r & 127u, XGM_HDR_TF_BITS(bh.meta));
-                    /* MultiAndPostList::get_weight: result += plist[i]->get_weight(), in plist order */
-                    acc[0] = __dadd_rn(acc[0], bm25_sumpart(q->terms[j].termweight, q, tfj, dlen));
-                }
-                if (q->nmaybe) { /* OP_AND_MAYBE: res = l; if (r matches) res += r */
-                    const double rw = maybe_weight(p, q, d, dlen, &opt);
-                    if (opt) acc[0] = __dadd_rn(acc[0], rw);
-                }
-            }
-            const uint32_t cc[4] = {d, 0u, 0u, 0u};
-            const uint32_t nw = q->nweighted;
-            const uint32_t aux[4] = {nw + opt, nw, nw, nw};
-            emit_matches(p, q, wi.query, lane, alive, acc, cc, aux);
-        };
-        auto issue = [&](uint32_t b, uint32_t blk) { /* stage driver block blk into buffer b */
-            const XgmBlockHdr h = hdr[drv_begin + blk];
-            const uint32_t bits = XGM_HDR_DOC_BITS(h.meta);
-            __syncwarp();
-            if (bits != 0 && lane == 0) {
-                mbar_expect_tx_a(bar_base + b * 8u, bits * 16u);
-                bulk_g2s_a(stage_base + b * (STAGE_WORDS * 4u), p.docs + h.doc_off, bits * 16u, bar_base + b * 8u);
-            }
-            return h;
-        };
-
-        XgmBlockHdr h0 = issue(0, wi.b0), h1 = h0;
-        if (wi.b0 + 1 < wi.b1) h1 = issue(1, wi.b0 + 1);
-        uint32_t cur = 0; /* buffers cur, cur+1 hold the current pair; (cur^2), (cur^2)+1 the next */
-        for (uint32_t db = wi.b0; db < wi.b1; db += 2) {
-            const bool two = db + 1 < wi.b1;
-            XgmBlockHdr n0 = h0, n1 = h1;
-            if (db + 2 < wi.b1) n0 = issue(cur ^ 2, db + 2);
-            if (db + 3 < wi.b1) n1 = issue((cur ^ 2) + 1, db + 3);
-            uint32_t c[8];
-            uint32_t alive;
-            const uint32_t cnt0 = XGM_HDR_COUNT(h0.meta), cnt1 = two ? XGM_HDR_COUNT(h1.meta) : 0u;
-            {
-                const uint32_t bits = XGM_HDR_DOC_BITS(h0.meta);
-                if (bits) { mbar_wait_a(bar_base + cur * 8u, (phases >> cur) & 1u); phases ^= 1u << cur; }
-                decode_docids(ws.dstage[cur], bits, h0.first, lane, c);
-            }
-            if (two) {
-                const uint32_t bits = XGM_HDR_DOC_BITS(h1.meta);
-                if (bits) { mbar_wait_a(bar_base + (cur + 1) * 8u, (phases >> (cur + 1)) & 1u); phases ^= 1u << (cur + 1); }
-                decode_docids(ws.dstage[cur + 1], bits, h1.first, lane, c + 4);
-            } else {
-                c[4] = c[5] = c[6] = c[7] = 0u;
-            }
-            /* the skip_to/check of the leapfrog: one bitmap word per candidate, all loads issued together */
-            uint32_t w[8];
-            if (cnt0 + cnt1 == 2u * XGM_BLOCK) { /* two full blocks (warp-uniform): no per-posting predicates */
-                alive = 0xffu;
-#pragma unroll
-                for (int k = 0; k < 8; ++k) w[k] = __ldg(bm1 + (c[k] >> 5));
-            } else {
-                const int n0 = min(4, max(0, (int)cnt0 - 4 * (int)lane)), n1 = min(4, max(0, (int)cnt1 - 4 * (int)lane));
-                alive = ((1u << n0) - 1u) | (((1u << n1) - 1u) << 4);
-#pragma unroll
-                for (int k = 0; k < 8; ++k) w[k] = (alive >> k & 1u) ? __ldg(bm1 + (c[k] >> 5)) : 0u;
-            }
-            uint32_t surv = 0; /* dead slots carry w = 0 */
-#pragma unroll
-            for (int k = 0; k < 8; ++k) surv |= (__funnelshift_r(w[k], 0u, c[k]) & 1u) << k; /* shifts by c & 31 */
-            if (__any_sync(FULL, surv != 0)) {
-                /* survivors are rare (a few per pair of blocks): one ballot per slot, empty slots skipped */
-                const uint32_t lt = (1u << lane) - 1u;
-#pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    const bool mine = surv >> k & 1u;
-                    const uint32_t b = __ballot_sync(FULL, mine);
-                    if (b) {
-                        if (mine) {
-                            const uint32_t slot = qn + __popc(b & lt);
-                            ws.qdid[slot] = c[k];
-                            ws.qsrc[slot] = ((db - wi.b0 + (k >> 2)) << 7) | (4 * lane + (k & 3));
-                        }
-                        qn += __popc(b);
-                    }
-                }
-                __syncwarp();
-                while (qn >= 32) {
-                    qn -= 32;
-                    flush(qn, 32);
-                    __syncwarp();
-                }
-            }
-            h0 = n0;
-            h1 = n1;
-            cur ^= 2u;
-        }
-        if (qn) {
-            flush(0, qn);
-            __syncwarp();
-        }
-    }
-}
-
-#undef bar_base
-
-/* ------------------------------------------------------------------ bitmap AND kernel, two-stage queues */
-
-/* Same contract as xgm_and_bm_kernel.  What changed is where the rare work happens.  Of the driver postings
- * ~1 % pass the second list's bitmap and ~0.01 % are matches, yet in the kernel above every work item ended
- * with a partially filled flush that ran the whole scoring code (two rank look-ups, three wdf unpacks, three
- * f64 divisions, emission) for a handful of live lanes.  Here a warp keeps two queues in shared memory for
- * its whole lifetime, entries tagged with their query:
+ * path so that more warps fit an SM (the kernel is bound by the latency of the bitmap probes): a warp
+ * decodes TWO driver blocks at a time (bulk copies of the next pair already in flight) and issues the 8
+ * bitmap word loads of every lane together.  Of the driver postings ~1 % pass the second list's bitmap
+ * and ~0.01 % are matches, so the rare work is queued: a warp keeps two queues in shared memory for its
+ * whole lifetime, entries tagged with their query:
  *   stage 1  candidates confirmed by the second list       → flushed 32 at a time: remaining bitmaps
  *            (required / excluded lists), value-range predicate; the survivors — the matches — go to
  *   stage 2  matches                                       → flushed 32 at a time: rank → wdf, doc length,
@@ -1019,13 +853,14 @@ __global__ void __launch_bounds__(BM_WARPS * 32, 4) xgm_and_bm_kernel(XgmKernelP
 
 struct __align__(16) Bm3Scratch {
     uint32_t dstage[4][STAGE_WORDS]; /* packed driver blocks (bulk copies), then their decoded docids */
-    uint32_t q1did[BM3_Q1CAP]; /* stage 1 belongs to the current work item (one query) */
-    uint16_t q1src[BM3_Q1CAP]; /* (driver block - b0) << 7 | position */
+    uint32_t q1did[BM3_Q1CAP]; /* stage 1 belongs to the current work item (one run of queries) */
+    uint16_t q1src[BM3_Q1CAP]; /* query slot << 12 | (driver block - b0) << 7 | position (b1 - b0 <= 32) */
     uint32_t q2did[BM3_Q2CAP]; /* stage 2 lives as long as the warp: entries carry their query */
     uint32_t q2src[BM3_Q2CAP]; /* index of the driver block's header in hdr[] */
     uint32_t q2qi[BM3_Q2CAP];  /* query | position in the driver block << 25 */
     uint64_t dbar[4];
 };
+static_assert(XGM_BM_RUN <= 16, "q1src keeps a query slot in 4 bits");
 /* 4.6 KB per warp, 37 KB per CTA: with 4 CTAs per SM the shared-memory carve-out stays at 164 KB and the
  * bitmap probes keep ~90 KB of L1 (51 KB per CTA would push the carve-out to 228 KB and leave the probes
  * almost no L1). */
@@ -1112,68 +947,20 @@ __device__ __forceinline__ void emit_match_lanes(const XgmKernelParams& p, uint3
     }
 }
 
-/* Next non-empty group of the grouped bitmap AND list (work_counter[6] counts them), packed as end << 32 | first
- * item; 0: none left. */
-__device__ __noinline__ unsigned long long bm3_fetch_group(const XgmKernelParams& p, uint32_t nitems_bm) {
-    for (;;) {
-        const uint32_t g = atomicAdd(p.work_counter + 6, 1u);
-        if (g >= p.ngroups) return 0ull;
-        const uint32_t a = __ldg(p.grp_off + g), b = g + 1 < p.ngroups ? __ldg(p.grp_off + g + 1) : nitems_bm;
-        if (a < b) return (unsigned long long)b << 32 | a;
-    }
-}
-
-/* Next item of the grouped bitmap AND list for the calling lane's warp (one lane per warp; nitems_bm: no work
- * left).  cur holds the CTA's current group, items [low word, high word), and next the group after it (~0 while
- * it is being fetched).  No warp waits for another to finish its item: the warp whose claim equals the end
- * installs the next group and fetches the one after; the others spin for the short time that takes.  Kept out of
- * line so that the pair step keeps its registers. */
-__device__ __noinline__ uint32_t bm3_claim_grouped(const XgmKernelParams& p, uint32_t nitems_bm, unsigned long long* cur,
-                                                   unsigned long long* next) {
-    volatile unsigned long long* vcur = cur;
-    volatile unsigned long long* vnext = next;
-    for (;;) {
-        const unsigned long long cw = atomicAdd(cur, 1ull);
-        const uint32_t nx = (uint32_t)cw, en = (uint32_t)(cw >> 32);
-        if (nx < en) return nx;
-        if (nx == en) {
-            unsigned long long n;
-            while ((n = *vnext) == ~0ull) __nanosleep(32); /* the previous installer is still fetching */
-            if (n == 0ull) return nitems_bm; /* cur stays used up: every later claim ends here too */
-            *vnext = ~0ull; /* not to be installed twice */
-            __threadfence_block();
-            *vcur = n + 1u; /* this warp takes the group's first item */
-            *vnext = bm3_fetch_group(p, nitems_bm);
-            return (uint32_t)n;
-        }
-        for (;;) {
-            const unsigned long long v = *vcur;
-            if ((uint32_t)v < (uint32_t)(v >> 32)) break;
-            if (*vnext == 0ull) return nitems_bm;
-            __nanosleep(32);
-        }
-    }
-}
-
-/* One flat loop with four states, so that each piece of code exists once and nothing is called from the hot
+/* One flat loop with five states, so that each piece of code exists once and nothing is called from the hot
  * path: score 32 matches (stage 2 full, or out of work) → finish 32 candidates (stage 1 full, or the item
- * ended) → fetch the next work item → decode and probe the next pair of driver blocks. */
+ * ended) → fetch the next work item → probe the decoded pair of driver blocks for the next query slot of the
+ * item's run → decode the next pair.  A pair is decoded once and probed once per query of the run. */
 template <int MINB>
 __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const __grid_constant__ XgmKernelParams p) {
     extern __shared__ __align__(16) unsigned char bm3_raw[];
     Bm3Scratch* scratch = reinterpret_cast<Bm3Scratch*>(bm3_raw);
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     Bm3Scratch& ws = scratch[warp];
-    /* grouped list (p.ngroups != 0): the CTA's current group and the next one (bm3_claim_grouped) */
-    __shared__ unsigned long long grp_cur, grp_next;
     if (lane < 4) mbar_init(&ws.dbar[lane], 1);
-    if (threadIdx.x == 0) {
-        grp_cur = 0;
-        if (p.ngroups != 0) grp_next = bm3_fetch_group(p, p.nitems_bm_dev ? __ldg(p.nitems_bm_dev) : p.nitems_bm);
-    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
-    uint32_t phases = 0;
+    uint32_t phases = 0; /* bits 0-3: mbarrier phase of each buffer; bits 8-16: the decoded pair's alive bits (below) */
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
     const uint32_t stage_base = smem_u32(ws.dstage[0]);
     const uint32_t bar_base = stage_base + (uint32_t)offsetof(Bm3Scratch, dbar);
@@ -1181,15 +968,18 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
     const uint32_t nitems_bm = p.nitems_bm_dev ? __ldg(p.nitems_bm_dev) : p.nitems_bm;
     uint32_t qn1 = 0, qn2 = 0; /* warp-uniform queue lengths */
     bool done = false;
-    /* current work item: driver blocks [db, it_b1) of query it_query are left (db >= it_b1: none) */
-    uint32_t it_query = 0, it_b0 = 0, it_b1 = 0, db = 0, drv_begin = 0, cur = 0;
-    const XgmDevQuery* q = p.queries;
-    const uint32_t* __restrict__ bm1 = p.bitmaps;
+    /* current work item: its driver blocks are hdr[drv + i], i < it_n; those from db on are left to decode */
+    uint32_t drv = 0, it_n = 0, db = 0, cur = 0;
+    /* the item's run: lane s holds the query of slot s and the offset of its probe bitmap (terms[1]).  run_bits: low
+     * half, a bit per slot that takes part (in the second pass only the queries that re-run); high half, the slots
+     * still to probe on the decoded pair, which sits in buffers cur ^ 2, cur ^ 2 + 1 */
+    uint32_t slot_q = 0, run_bits = 0;
+    uint64_t slot_bm = 0;
     uint2 h0 = make_uint2(0u, 0u), h1 = h0; /* (first docid, meta) of the staged pair */
 
     /* stage driver block blk into buffer b; only (first docid, meta) of its header stay live */
     auto issue = [&](uint32_t b, uint32_t blk) {
-        const uint4 h = __ldg(reinterpret_cast<const uint4*>(hdr + drv_begin + blk));
+        const uint4 h = __ldg(reinterpret_cast<const uint4*>(hdr + drv + blk));
         const uint32_t bits = XGM_HDR_DOC_BITS(h.w);
         __syncwarp();
         if (bits != 0 && lane == 0) {
@@ -1239,7 +1029,7 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
             __syncwarp();
             continue;
         }
-        const bool item_end = db >= it_b1;
+        const bool item_end = db >= it_n && (run_bits >> 16) == 0;
         /* ---- stage 1: finish the boolean test of queued candidates of the current item ---- */
         if (qn1 >= 32 || (item_end && qn1 != 0)) {
             __syncwarp();
@@ -1248,9 +1038,12 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
             bool alive = lane < count;
             const uint32_t d = alive ? ws.q1did[qn1 + lane] : 0u;
             const uint32_t src = alive ? ws.q1src[qn1 + lane] : 0u;
+            /* the lanes' candidates belong to different queries of the run */
+            const uint32_t qi = __shfl_sync(FULL, slot_q, src >> 12);
+            const XgmDevQuery* q = &p.queries[qi];
             const uint32_t nterms = q->nterms, nall = nterms + q->nnot;
-            for (uint32_t j = 2; j < nall && __any_sync(FULL, alive); ++j) {
-                if (alive) {
+            for (uint32_t j = 2; __any_sync(FULL, alive && j < nall); ++j) {
+                if (alive && j < nall) {
                     const uint32_t w = __ldg(p.bitmaps + q->terms[j].bm_off + (d >> 5));
                     /* required lists must hold the docid; the right side of an OP_AND_NOT must not
                      * (AndNotPostList::next, matcher/andnotpostlist.cc:97-130) */
@@ -1262,8 +1055,8 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
             if (alive) {
                 const uint32_t slot = qn2 + __popc(m & ((1u << lane) - 1u));
                 ws.q2did[slot] = d;
-                ws.q2src[slot] = drv_begin + it_b0 + (src >> 7);
-                ws.q2qi[slot] = it_query | ((src & 127u) << 25);
+                ws.q2src[slot] = drv + ((src >> 7) & 31u);
+                ws.q2qi[slot] = qi | ((src & 127u) << 25);
             }
             qn2 += __popc(m);
             __syncwarp();
@@ -1273,73 +1066,46 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
         /* ---- next work item ---- */
         if (item_end) {
             uint32_t item = 0;
-            if (p.ngroups == 0) {
-                if (lane == 0) item = atomicAdd(p.work_counter + 6 + p.pass, 1u);
-            } else if (lane == 0) {
-                /* the queries of a group probe the same bitmap in the same docid range: the CTA's warps share L1 lines */
-                item = bm3_claim_grouped(p, nitems_bm, &grp_cur, &grp_next);
-            }
+            if (lane == 0) item = atomicAdd(p.work_counter + 6 + p.pass, 1u);
             item = __shfl_sync(FULL, item, 0);
             if (item >= nitems_bm) { done = true; continue; }
             const XgmWorkItem wi = p.items_bm[item];
-            if (p.pass != 0 && p.qstate[wi.query].rerun == 0) continue;
-            it_query = wi.query; it_b0 = wi.b0; it_b1 = wi.b1; db = wi.b0;
-            q = &p.queries[wi.query];
-            drv_begin = q->terms[0].blk_begin;
-            bm1 = p.bitmaps + q->terms[1].bm_off;
-            h0 = issue(0, db);
+            const uint32_t n = p.bm_segs ? wi.pad : 1u;
+            slot_q = lane >= n ? 0u : p.bm_segs ? p.bm_segs[wi.query + lane].query : wi.query;
+            const bool take = lane < n && (p.pass == 0 || p.qstate[slot_q].rerun != 0);
+            run_bits = __ballot_sync(FULL, take);
+            if (run_bits == 0) continue; /* second pass: no query of the run re-runs */
+            slot_bm = take ? p.queries[slot_q].terms[1].bm_off : 0ull;
+            drv = p.queries[__shfl_sync(FULL, slot_q, 0)].terms[0].blk_begin + wi.b0;
+            it_n = wi.b1 - wi.b0;
+            db = 0;
+            /* buffers 0 and 1 may hold the last item's pair, read by the generic proxy; the bulk copies refill them */
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            h0 = issue(0, 0);
             h1 = h0;
-            if (db + 1 < it_b1) h1 = issue(1, db + 1);
+            if (it_n > 1) h1 = issue(1, 1);
             cur = 0; /* buffers cur, cur+1 hold the current pair; (cur^2), (cur^2)+1 the next */
             continue;
         }
-        /* ---- one pair of driver blocks ---- */
-        {
-            const bool two = db + 1 < it_b1;
-            uint2 n0 = h0, n1 = h1;
-            if (db + 2 < it_b1) n0 = issue(cur ^ 2, db + 2);
-            if (db + 3 < it_b1) n1 = issue((cur ^ 2) + 1, db + 3);
+        /* ---- probe the decoded pair for one query slot of the run ---- */
+        if ((run_bits >> 16) != 0) {
+            const uint32_t s = (uint32_t)__ffs(run_bits >> 16) - 1u;
+            run_bits ^= 1u << (16 + s);
+            const uint32_t* __restrict__ bm1 = p.bitmaps + __shfl_sync(FULL, slot_bm, s);
+            const uint32_t pb = cur ^ 2u;
+            /* slot k of lane l: posting 32 (k & 3) + l of block k >> 2, as the decode step left it */
             uint32_t c[8];
-            uint32_t alive;
-            const uint32_t cnt0 = XGM_HDR_COUNT(h0.y), cnt1 = two ? XGM_HDR_COUNT(h1.y) : 0u;
-            {
-                const uint32_t bits = XGM_HDR_DOC_BITS(h0.y);
-                if (bits) { mbar_wait_a(bar_base + cur * 8u, (phases >> cur) & 1u); phases ^= 1u << cur; }
-                decode_docids(ws.dstage[cur], bits, h0.x, lane, c);
-            }
-            if (two) {
-                const uint32_t bits = XGM_HDR_DOC_BITS(h1.y);
-                if (bits) { mbar_wait_a(bar_base + (cur + 1) * 8u, (phases >> (cur + 1)) & 1u); phases ^= 1u << (cur + 1); }
-                decode_docids(ws.dstage[cur + 1], bits, h1.x, lane, c + 4);
-            } else {
-                c[4] = c[5] = c[6] = c[7] = 0u;
-            }
-            /* Interleave the postings across the lanes, through the staging buffers they were decoded from: after
-             * this, slot k of lane l holds posting 32 (k & 3) + l of block k >> 2.  decode_docids leaves a lane
-             * postings 4l..4l+3, at C2's driver density ~85 bytes of bitmap from its neighbour's, so each probe load
-             * below would touch ~21 cache lines per warp; interleaved, its 32 lanes are 32 consecutive postings.  (An
-             * absent second block transposes its zeros.)  The bulk-copy engine refills these buffers for a later
-             * pair: the proxy fence orders this generic-proxy write before that async-proxy one. */
-            __syncwarp();
-            reinterpret_cast<uint4*>(ws.dstage[cur])[lane] = make_uint4(c[0], c[1], c[2], c[3]);
-            reinterpret_cast<uint4*>(ws.dstage[cur + 1])[lane] = make_uint4(c[4], c[5], c[6], c[7]);
-            __syncwarp();
 #pragma unroll
-            for (int k = 0; k < 8; ++k) c[k] = ws.dstage[cur + (k >> 2)][32 * (k & 3) + lane];
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            for (int k = 0; k < 8; ++k) c[k] = ws.dstage[pb + (k >> 2)][32 * (k & 3) + lane];
             /* the skip_to/check of the leapfrog: one bitmap word per candidate, all loads issued together */
             uint32_t w[8];
-            if (cnt0 + cnt1 == 2u * XGM_BLOCK) { /* two full blocks (warp-uniform): no per-posting predicates */
-                alive = 0xffu;
+            /* phases >> 8, bit k: this lane's slot k holds a posting; bit 8: both blocks are full (warp-uniform) */
+            if (phases >> 16) { /* two full blocks: no per-posting predicates */
 #pragma unroll
                 for (int k = 0; k < 8; ++k) w[k] = __ldg(bm1 + (c[k] >> 5));
             } else {
-                /* slot k < 4 holds posting 32k + lane of the first block: the lane has (cnt + 31 - lane) / 32 of
-                 * each block's cnt postings (cnt <= 128, and 0 of an absent second block) */
-                const uint32_t m0 = (cnt0 + 31u - lane) >> 5, m1 = (cnt1 + 31u - lane) >> 5;
-                alive = ((1u << m0) - 1u) | (((1u << m1) - 1u) << 4);
 #pragma unroll
-                for (int k = 0; k < 8; ++k) w[k] = (alive >> k & 1u) ? __ldg(bm1 + (c[k] >> 5)) : 0u;
+                for (int k = 0; k < 8; ++k) w[k] = (phases >> (8 + k) & 1u) ? __ldg(bm1 + (c[k] >> 5)) : 0u;
             }
             uint32_t surv = 0; /* dead slots carry w = 0 */
 #pragma unroll
@@ -1356,7 +1122,7 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
                 if (surv) {
                     const uint32_t lt = (1u << lane) - 1u;
                     uint32_t slot = qn1 + __popc(B & lt) + __popc(B0 & lt) + 2u * __popc(B1 & lt) + 4u * __popc(B2 & lt);
-                    const uint32_t rb = (db - it_b0) << 7 | lane;
+                    const uint32_t rb = s << 12 | (db - 2u) << 7 | lane; /* db has moved on to the next pair */
 #pragma unroll
                     for (int k = 0; k < 8; ++k)
                         if (surv >> k & 1u) {
@@ -1367,6 +1133,50 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
                 }
                 qn1 += __popc(B) + __popc(B0) + 2u * __popc(B1) + 4u * __popc(B2);
             }
+            continue;
+        }
+        /* ---- decode the next pair of driver blocks ---- */
+        {
+            const bool two = db + 1 < it_n;
+            /* the probes read buffers cur ^ 2 through the generic proxy; the bulk copies below refill them */
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            uint2 n0 = h0, n1 = h1;
+            if (db + 2 < it_n) n0 = issue(cur ^ 2, db + 2);
+            if (db + 3 < it_n) n1 = issue((cur ^ 2) + 1, db + 3);
+            uint32_t c[8];
+            const uint32_t cnt0 = XGM_HDR_COUNT(h0.y), cnt1 = two ? XGM_HDR_COUNT(h1.y) : 0u;
+            {
+                const uint32_t bits = XGM_HDR_DOC_BITS(h0.y);
+                if (bits) { mbar_wait_a(bar_base + cur * 8u, (phases >> cur) & 1u); phases ^= 1u << cur; }
+                decode_docids(ws.dstage[cur], bits, h0.x, lane, c);
+            }
+            if (two) {
+                const uint32_t bits = XGM_HDR_DOC_BITS(h1.y);
+                if (bits) { mbar_wait_a(bar_base + (cur + 1) * 8u, (phases >> (cur + 1)) & 1u); phases ^= 1u << (cur + 1); }
+                decode_docids(ws.dstage[cur + 1], bits, h1.x, lane, c + 4);
+            } else {
+                c[4] = c[5] = c[6] = c[7] = 0u;
+            }
+            /* Interleave the postings across the lanes, through the staging buffers they were decoded from: the
+             * probe step reads slot k of lane l as posting 32 (k & 3) + l of block k >> 2.  decode_docids leaves a
+             * lane postings 4l..4l+3, at C2's driver density ~85 bytes of bitmap from its neighbour's, so each probe
+             * load would touch ~21 cache lines per warp; interleaved, its 32 lanes are 32 consecutive postings.  (An
+             * absent second block transposes its zeros.)  The buffers are not refilled before every slot of the run
+             * has probed them: the next pair's decode issues into the other two. */
+            __syncwarp();
+            reinterpret_cast<uint4*>(ws.dstage[cur])[lane] = make_uint4(c[0], c[1], c[2], c[3]);
+            reinterpret_cast<uint4*>(ws.dstage[cur + 1])[lane] = make_uint4(c[4], c[5], c[6], c[7]);
+            __syncwarp();
+            phases &= 0xffu;
+            if (cnt0 + cnt1 == 2u * XGM_BLOCK) {
+                phases |= 0x1ffu << 8;
+            } else {
+                /* slot k < 4 holds posting 32k + lane of the first block: the lane has (cnt + 31 - lane) / 32 of
+                 * each block's cnt postings (cnt <= 128, and 0 of an absent second block) */
+                const uint32_t m0 = (cnt0 + 31u - lane) >> 5, m1 = (cnt1 + 31u - lane) >> 5;
+                phases |= (((1u << m0) - 1u) | (((1u << m1) - 1u) << 4)) << 8;
+            }
+            run_bits = (run_bits & 0xffffu) * 0x10001u; /* every slot probes the pair */
             h0 = n0;
             h1 = n1;
             cur ^= 2u;
@@ -1375,12 +1185,12 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
     }
 }
 
-static int g_bm_variant = -1; /* XGM_BM_VARIANT: 1 = one-stage kernel above; 33/34/35 = two-stage with launch bounds for 3/4/5 CTAs per SM */
+static int g_bm_variant = -1; /* XGM_BM_VARIANT: 33/34/35 = launch bounds for 3/4/5 CTAs per SM */
 static int bm_variant() {
     if (g_bm_variant < 0) {
         const char* e = getenv("XGM_BM_VARIANT");
         g_bm_variant = e ? atoi(e) : 34;
-        if (g_bm_variant != 1 && (g_bm_variant < 33 || g_bm_variant > 35)) g_bm_variant = 34;
+        if (g_bm_variant < 33 || g_bm_variant > 35) g_bm_variant = 34;
     }
     return g_bm_variant;
 }
@@ -1391,12 +1201,7 @@ static bm3_fn bm3_kernel(int v) {
 }
 
 cudaError_t xgm_launch_and_bm(const XgmKernelParams& p, int grid, cudaStream_t s) {
-    const int v = bm_variant();
-    if (v == 1) {
-        xgm_and_bm_kernel<<<grid, BM_WARPS * 32, 0, s>>>(p);
-    } else {
-        bm3_kernel(v)<<<grid, BM3_WARPS * 32, sizeof(Bm3Scratch) * BM3_WARPS, s>>>(p);
-    }
+    bm3_kernel(bm_variant())<<<grid, BM3_WARPS * 32, sizeof(Bm3Scratch) * BM3_WARPS, s>>>(p);
     return cudaGetLastError();
 }
 
@@ -1404,14 +1209,10 @@ cudaError_t xgm_launch_and_bm(const XgmKernelParams& p, int grid, cudaStream_t s
  * call once per searcher, after cudaSetDevice). */
 int xgm_and_bm_occupancy_blocks_per_sm() {
     int n = 0;
-    const int v = bm_variant();
-    if (v == 1) {
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_and_bm_kernel, BM_WARPS * 32, 0);
-    } else {
-        const size_t smem = sizeof(Bm3Scratch) * BM3_WARPS;
-        cudaFuncSetAttribute(bm3_kernel(v), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, bm3_kernel(v), BM3_WARPS * 32, smem);
-    }
+    const bm3_fn f = bm3_kernel(bm_variant());
+    const size_t smem = sizeof(Bm3Scratch) * BM3_WARPS;
+    cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, f, BM3_WARPS * 32, smem);
     return n;
 }
 
@@ -3234,7 +3035,8 @@ __global__ void xgm_expand_items_kernel(const XgmWorkItem* __restrict__ seg, uin
  * bitmap (lastdocid/8 bytes per term shrink to 2^range_bits/8), which stays in the 50 MB L2 while the
  * whole batch walks over it — each bitmap is read from HBM about once per batch instead of once per query
  * that uses it.  Every query still advances through the whole batch, so thresholds rise early as with the
- * level order.  Three small kernels: per (range, segment) the driver blocks whose first docid falls in
+ * level order.  The list's unit is a run of up to XGM_BM_RUN queries with the same driver list: its items
+ * serve all of them.  Three small kernels: per (range, run) the driver blocks whose first docid falls in
  * the range (two binary searches over the skip table) and their item count; an exclusive scan in
  * range-major order; the fill. */
 __device__ __forceinline__ uint32_t first_block_at_or_after(const XgmBlockHdr* __restrict__ h, uint32_t nblk, uint64_t target) {
@@ -3269,17 +3071,17 @@ __device__ __forceinline__ uint32_t block_exclusive_scan_256(uint32_t v, uint32_
 }
 
 __global__ void __launch_bounds__(XGM_RNG_THREADS) xgm_range_count_kernel(
-    const XgmWorkItem* __restrict__ seg, uint32_t nseg, const XgmDevQuery* __restrict__ queries,
-    const XgmBlockHdr* __restrict__ hdr, uint32_t nranges, uint32_t range_bits, uint32_t bpi, uint32_t* __restrict__ lo_out,
-    uint32_t* __restrict__ cnt_out, uint32_t* __restrict__ block_sums) {
+    const XgmWorkItem* __restrict__ runs, uint32_t nruns, const XgmBlockHdr* __restrict__ hdr, uint32_t nranges,
+    uint32_t range_bits, uint32_t bpi, uint32_t* __restrict__ lo_out, uint32_t* __restrict__ cnt_out,
+    uint32_t* __restrict__ block_sums) {
     __shared__ uint32_t warp_sums[XGM_RNG_THREADS / 32];
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t cnt = 0;
-    if (t < nranges * nseg) {
-        const uint32_t j = t / nseg, sidx = t - j * nseg; /* range-major: consecutive threads = consecutive segments */
-        const XgmWorkItem sg = seg[sidx];
-        const XgmBlockHdr* h = hdr + queries[sg.query].terms[0].blk_begin;
-        const uint32_t nblk = sg.b0;
+    if (t < nranges * nruns) {
+        const uint32_t j = t / nruns, r = t - j * nruns; /* range-major: consecutive threads = consecutive runs */
+        const XgmWorkItem rn = runs[r]; /* b0 = #driver blocks, b1 = the driver's first header */
+        const XgmBlockHdr* h = hdr + rn.b1;
+        const uint32_t nblk = rn.b0;
         /* a block belongs to the range of its first docid */
         const uint32_t lo = j == 0 ? 0u : first_block_at_or_after(h, nblk, (uint64_t)j << range_bits);
         const uint32_t hi = j + 1 == nranges ? nblk : first_block_at_or_after(h, nblk, (uint64_t)(j + 1) << range_bits);
@@ -3316,26 +3118,22 @@ __global__ void __launch_bounds__(XGM_SCAN_THREADS) xgm_range_scan_kernel(uint32
 }
 
 __global__ void __launch_bounds__(XGM_RNG_THREADS) xgm_range_fill_kernel(
-    const XgmWorkItem* __restrict__ seg, uint32_t nseg, uint32_t nranges, uint32_t bpi, const uint32_t* __restrict__ lo_in,
-    const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ block_off, XgmWorkItem* __restrict__ out,
-    uint32_t nruns, uint32_t* __restrict__ grp_off) {
+    const XgmWorkItem* __restrict__ runs, uint32_t nruns, uint32_t nranges, uint32_t bpi, const uint32_t* __restrict__ lo_in,
+    const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ block_off, XgmWorkItem* __restrict__ out) {
     __shared__ uint32_t warp_sums[XGM_RNG_THREADS / 32];
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    const bool in = t < nranges * nseg;
+    const bool in = t < nranges * nruns;
     const uint32_t n = in ? cnt[t] : 0u;
     uint32_t total;
     const uint32_t off = block_off[blockIdx.x] + block_exclusive_scan_256(n, warp_sums, &total);
-    if (!in) return;
-    const uint32_t j = t / nseg, sidx = t - j * nseg;
-    const XgmWorkItem sg = seg[sidx];
-    /* the first segment of run r (pad = 0x80000000 | r) starts group (j, r) */
-    if (grp_off != nullptr && (sg.pad >> 31) != 0) grp_off[j * nruns + (sg.pad & 0x7fffffffu)] = off;
-    if (n == 0) return;
+    if (!in || n == 0) return;
+    const uint32_t j = t / nruns, r = t - j * nruns;
+    const XgmWorkItem rn = runs[r];
     const uint32_t lo = lo_in[t];
-    const uint32_t hi = j + 1 == nranges ? sg.b0 : lo_in[t + nseg];
+    const uint32_t hi = j + 1 == nranges ? rn.b0 : lo_in[t + nruns];
     XgmWorkItem w;
-    w.query = sg.query;
-    w.pad = sg.pad;
+    w.query = rn.query; /* the run's first segment */
+    w.pad = rn.pad;     /* and its number of queries */
     for (uint32_t i = 0; i < n; ++i) {
         w.b0 = lo + i * bpi;
         w.b1 = min(hi, w.b0 + bpi);
@@ -3343,16 +3141,15 @@ __global__ void __launch_bounds__(XGM_RNG_THREADS) xgm_range_fill_kernel(
     }
 }
 
-cudaError_t xgm_launch_expand_ranges(const XgmWorkItem* seg, uint32_t nseg, const XgmDevQuery* queries, const XgmBlockHdr* hdr,
-                                     uint32_t nranges, uint32_t range_bits, uint32_t bpi, uint32_t* lo, uint32_t* cnt,
-                                     uint32_t* off, uint32_t* total, XgmWorkItem* out, uint32_t nruns, uint32_t* grp_off,
-                                     cudaStream_t s) {
-    const uint32_t n = nranges * nseg;
+cudaError_t xgm_launch_expand_ranges(const XgmWorkItem* runs, uint32_t nruns, const XgmBlockHdr* hdr, uint32_t nranges,
+                                     uint32_t range_bits, uint32_t bpi, uint32_t* lo, uint32_t* cnt, uint32_t* off,
+                                     uint32_t* total, XgmWorkItem* out, cudaStream_t s) {
+    const uint32_t n = nranges * nruns;
     if (n == 0) return cudaSuccess;
     const uint32_t nb = (n + XGM_RNG_THREADS - 1) / XGM_RNG_THREADS; /* `off` holds the nb block sums / offsets */
-    xgm_range_count_kernel<<<nb, XGM_RNG_THREADS, 0, s>>>(seg, nseg, queries, hdr, nranges, range_bits, bpi, lo, cnt, off);
+    xgm_range_count_kernel<<<nb, XGM_RNG_THREADS, 0, s>>>(runs, nruns, hdr, nranges, range_bits, bpi, lo, cnt, off);
     xgm_range_scan_kernel<<<1, XGM_SCAN_THREADS, 0, s>>>(off, nb, total);
-    xgm_range_fill_kernel<<<nb, XGM_RNG_THREADS, 0, s>>>(seg, nseg, nranges, bpi, lo, cnt, off, out, nruns, grp_off);
+    xgm_range_fill_kernel<<<nb, XGM_RNG_THREADS, 0, s>>>(runs, nruns, nranges, bpi, lo, cnt, off, out);
     return cudaGetLastError();
 }
 
