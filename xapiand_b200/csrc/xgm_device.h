@@ -78,8 +78,6 @@ struct XgmKernelParams {
 #define XGM_CTRL_HDR 128 /* bytes of work counters in front of the per-query state */
 
 cudaError_t xgm_launch_and(const XgmKernelParams& p, int grid, cudaStream_t s);
-cudaError_t xgm_launch_and2(const XgmKernelParams& p, int grid, cudaStream_t s);
-int xgm_and2_occupancy_blocks_per_sm();
 cudaError_t xgm_launch_and_bm(const XgmKernelParams& p, int grid, cudaStream_t s);
 int xgm_and_bm_occupancy_blocks_per_sm();
 cudaError_t xgm_launch_expand(const XgmWorkItem* seg, uint32_t nseg, uint32_t total, const uint32_t* level_start,

@@ -916,6 +916,87 @@ struct PlannedQuery {
     bool log_raises = false; /* … and the MSet is not ordered by weight: subqueries of the best-weighted document come from the raise log */
 };
 
+/* A pinned host array and its device copy: the host fills it and one copy uploads it. */
+template <class T> struct PinnedPair {
+    T* h = nullptr;
+    T* d = nullptr;
+    size_t cap = 0;
+    /* room for `need` elements, grown to max(2 need, floor); the stream's copies and kernels may still read the
+     * old buffers, so it is waited for before they are freed */
+    xgm_status reserve(size_t need, size_t floor, cudaStream_t st) {
+        if (need <= cap) return XGM_OK;
+        const size_t c = std::max(need * 2, floor);
+        CUDA_TRY(cudaStreamSynchronize(st));
+        release();
+        CUDA_TRY(cudaMallocHost(&h, c * sizeof(T)));
+        CUDA_TRY(cudaMalloc(&d, c * sizeof(T)));
+        cap = c;
+        return XGM_OK;
+    }
+    cudaError_t upload(size_t n, cudaStream_t st) const {
+        return n ? cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, st) : cudaSuccess;
+    }
+    void release() {
+        if (h) cudaFreeHost(h);
+        cudaFree(d);
+        h = nullptr; d = nullptr; cap = 0;
+    }
+};
+
+/* One work list of a batch: a segment per query (per query and leaf on the OR list), which the device expands
+ * into work items of at most bpi driver blocks. */
+struct WorkList {
+    PinnedPair<XgmWorkItem> seg;  /* segments, in the order the expansion reads them */
+    PinnedPair<uint32_t> levels;  /* level starts of a level-ordered expansion */
+    XgmWorkItem* d_exp = nullptr; /* expanded + interleaved work items (device only) */
+    size_t exp_cap = 0;
+    uint32_t nseg = 0, nstarts = 0, nitems = 0; /* nstarts: entries of `levels` in use */
+    /* the segments expand to n work items: room for them on the device */
+    xgm_status set_items(uint64_t n, cudaStream_t st) {
+        if (n >= 0xffffffffull) return fail(XGM_E_INVALID, "too many work items in one batch");
+        nitems = (uint32_t)n;
+        if (n <= exp_cap) return XGM_OK;
+        const size_t c = std::max<size_t>(n * 2, 65536);
+        CUDA_TRY(cudaStreamSynchronize(st));
+        cudaFree(d_exp);
+        d_exp = nullptr; exp_cap = 0;
+        CUDA_TRY(cudaMalloc(&d_exp, c * sizeof(XgmWorkItem)));
+        exp_cap = c;
+        return XGM_OK;
+    }
+    /* the segments, `extra` rows stored after them, and the level starts */
+    cudaError_t upload(uint32_t extra, cudaStream_t st) const {
+        cudaError_t e = seg.upload((size_t)nseg + extra, st);
+        return e != cudaSuccess ? e : levels.upload(nstarts, st);
+    }
+    void release() { seg.release(); levels.release(); cudaFree(d_exp); }
+};
+
+/* The OR list: one level-ordered expansion per leaf position */
+struct OrList : WorkList {
+    struct Group { uint32_t seg_off, nseg, level_off, nlevels, out_off, total; };
+    std::vector<Group> groups;
+};
+
+/* The bitmap AND list.  In range-major order its segments are followed by runs of segments that share a driver
+ * list, and the device expands it per (range, run). */
+struct BmList : WorkList {
+    bool range_mode = false;
+    uint32_t nranges = 1, nruns = 0;
+    uint32_t* d_rng = nullptr; /* per (range, run) first block, item count, output offset */
+    size_t rng_cap = 0;
+    uint32_t* d_rng_total = nullptr; /* [0] = number of items */
+    uint32_t* h_rng_total = nullptr;
+    void release() {
+        WorkList::release();
+        cudaFree(d_rng); cudaFree(d_rng_total);
+        if (h_rng_total) cudaFreeHost(h_rng_total);
+    }
+};
+
+/* A batch's segments as planned, one vector per work list */
+struct PlannedSegments { std::vector<XgmWorkItem> and_list, or_list, bm_list; };
+
 struct xgm_searcher {
     const xgm_index* ix = nullptr;
     int device = 0; /* ix->device, kept so that freeing the searcher never reads an index already closed */
@@ -929,9 +1010,6 @@ struct xgm_searcher {
     bool shared_compute = true;
     /* pinned host staging */
     XgmDevQuery* h_queries = nullptr;
-    XgmWorkItem* h_items = nullptr;
-    XgmWorkItem* h_items_or = nullptr;
-    XgmWorkItem* h_items_bm = nullptr;
     double* h_out_w = nullptr;
     uint32_t* h_out_d = nullptr;
     uint64_t* h_out_k = nullptr;
@@ -940,31 +1018,15 @@ struct xgm_searcher {
     XgmRaise* d_raise = nullptr;
     XgmQState* h_qstate = nullptr; /* pinned: per-query state after the batch (raise-log lengths) */
     bool any_raise = false;
-    size_t items_cap = 0, items_or_cap = 0, items_bm_cap = 0;
     uint32_t keep_cap = 0;
     size_t ctrl_bytes = 0;
     /* device */
     XgmDevQuery* d_queries = nullptr;
-    XgmWorkItem* d_items = nullptr;
-    XgmWorkItem* d_items_or = nullptr;
-    XgmWorkItem* d_items_bm = nullptr;
-    XgmWorkItem* d_exp[3] = {nullptr, nullptr, nullptr}; /* expanded + interleaved work lists (device only) */
-    size_t exp_cap[3] = {0, 0, 0};
-    uint32_t nseg[3] = {0, 0, 0}, nlevels[3] = {0, 0, 0}, bpi = 16;
-    uint32_t* h_levels[3] = {nullptr, nullptr, nullptr}; /* pinned: level_start arrays of the AND lists */
-    uint32_t* d_levels[3] = {nullptr, nullptr, nullptr};
-    size_t levels_cap[3] = {0, 0, 0};
-    /* range-major expansion of the bitmap AND list (large batches): per (range, segment) first block, item
-     * count, output offset; [0] of d_rng_total = number of items */
-    uint32_t* d_rng = nullptr;
-    size_t rng_cap = 0;
-    uint32_t* d_rng_total = nullptr;
-    uint32_t* h_rng_total = nullptr;
-    bool range_mode = false;
-    uint32_t range_bits = 17, nranges = 1; /* XGM_RANGE_BITS: 2^17 docids per range (DESIGN.md §3.1) */
-    uint32_t nruns = 0;                    /* runs of segments with one driver list (uploaded after the segments) */
-    struct OrGroup { uint32_t seg_off, nseg, level_off, nlevels, out_off, total; };
-    std::vector<OrGroup> or_groups; /* OR list: one level-ordered expansion per leaf position */
+    WorkList and_list; /* general AND kernel */
+    OrList or_list;
+    BmList bm_list;    /* bitmap AND kernel */
+    uint32_t bpi = 16;
+    uint32_t range_bits = 17; /* XGM_RANGE_BITS: 2^17 docids per range (DESIGN.md §3.1) */
     uint32_t* d_topk_list = nullptr; /* [max_batch] queries left to the CTA-per-query top-k kernel */
     unsigned char* d_ctrl = nullptr; /* [XGM_CTRL_HDR B work counters][nq x XgmQState][nq x XGM_NBINS x u32] */
     double* d_match_w = nullptr;
@@ -982,10 +1044,10 @@ struct xgm_searcher {
     size_t slab_bytes = 0, slab_off_d = 0, slab_off_info = 0;
     /* last batch */
     std::vector<PlannedQuery> plan;
-    uint32_t nq = 0, nitems = 0, nitems_or = 0, nitems_bm = 0;
+    uint32_t nq = 0;
     bool pending = false, any_sort = false;
     xgm_batch_stats stats{};
-    int grid = 0, grid_or = 0, grid_or3 = 0, grid_tile = 0, grid_and2 = 0, grid_bm = 0;
+    int grid = 0, grid_or = 0, grid_or3 = 0, grid_tile = 0, grid_bm = 0;
     bool any_or_fast = false, any_or_slow = false;
     uint32_t* h_tileq = nullptr;  /* pinned: queries of the batch answered by the bitmap-union kernel */
     uint32_t* d_tileq = nullptr;
@@ -993,7 +1055,6 @@ struct xgm_searcher {
     bool device_only = false;     /* results stay on the device (xgm_searcher_set_results_on_device) */
     uint32_t bpi_override = 0;    /* XGM_BPI: driver blocks per work item for batches >= 256 (default 16) */
     bool or_tile = true;          /* XGM_OR_TILE=0: keep every fast OR query in the one-launch kernel */
-    int and_version = 1; /* 1 = warp-autonomous kernel, 2 = chunked CTA kernel (XGM_AND_KERNEL env) */
     XgmKernelParams params;
     /* xgm_search_submit_async: a worker thread plans and enqueues the batch while the caller scatters the
      * results of an earlier one */
@@ -1035,64 +1096,20 @@ extern "C" void xgm_searcher_free(xgm_searcher* s) {
     }
     cudaSetDevice(s->device);
     if (s->stream) cudaStreamSynchronize(s->stream);
-    cudaFreeHost(s->h_queries); cudaFreeHost(s->h_items); cudaFreeHost(s->h_items_or); cudaFreeHost(s->h_items_bm); cudaFreeHost(s->h_out_w); cudaFreeHost(s->h_out_d);
+    cudaFreeHost(s->h_queries); cudaFreeHost(s->h_out_w); cudaFreeHost(s->h_out_d);
     cudaFreeHost(s->h_out_k); cudaFreeHost(s->h_info); cudaFreeHost(s->h_raise); cudaFree(s->d_raise); cudaFreeHost(s->h_qstate); cudaFreeHost(s->h_tileq); cudaFree(s->d_tileq);
-    cudaFree(s->d_queries); cudaFree(s->d_items); cudaFree(s->d_items_or); cudaFree(s->d_items_bm); cudaFree(s->d_exp[0]); cudaFree(s->d_exp[1]); cudaFree(s->d_exp[2]);
-    for (int w = 0; w < 3; ++w) { if (s->h_levels[w]) cudaFreeHost(s->h_levels[w]); cudaFree(s->d_levels[w]); } cudaFree(s->d_ctrl); cudaFree(s->d_topk_list); cudaFree(s->d_match_w); cudaFree(s->d_match_d);
+    cudaFree(s->d_queries); s->and_list.release(); s->or_list.release(); s->bm_list.release();
+    cudaFree(s->d_ctrl); cudaFree(s->d_topk_list); cudaFree(s->d_match_w); cudaFree(s->d_match_d);
     cudaFree(s->d_match_k); cudaFree(s->d_pool_w); cudaFree(s->d_pool_d); cudaFree(s->d_pool_k); cudaFree(s->d_slab); cudaFree(s->d_out_k);
     if (s->ev0) cudaEventDestroy(s->ev0);
     if (s->ev1) cudaEventDestroy(s->ev1);
     if (s->ev2) cudaEventDestroy(s->ev2);
-    cudaFree(s->d_rng); cudaFree(s->d_rng_total);
-    if (s->h_rng_total) cudaFreeHost(s->h_rng_total);
     if (s->ev_in) cudaEventDestroy(s->ev_in);
     if (s->tr_h2d) cudaEventDestroy(s->tr_h2d);
     if (s->tr_out) cudaEventDestroy(s->tr_out);
     if (s->ev_done) cudaEventDestroy(s->ev_done);
     if (s->stream) cudaStreamDestroy(s->stream);
     delete s;
-}
-
-static xgm_status ensure_items(xgm_searcher* s, size_t need, int which) {
-    size_t& have = which == 1 ? s->items_or_cap : which == 2 ? s->items_bm_cap : s->items_cap;
-    XgmWorkItem*& h = which == 1 ? s->h_items_or : which == 2 ? s->h_items_bm : s->h_items;
-    XgmWorkItem*& d = which == 1 ? s->d_items_or : which == 2 ? s->d_items_bm : s->d_items;
-    if (need <= have) return XGM_OK;
-    size_t cap = std::max<size_t>(need * 2, 4096);
-    CUDA_TRY(cudaStreamSynchronize(s->stream));
-    XgmWorkItem* nh = nullptr;
-    CUDA_TRY(cudaMallocHost(&nh, cap * sizeof(XgmWorkItem)));
-    if (h) cudaFreeHost(h);
-    h = nh;
-    cudaFree(d);
-    d = nullptr;
-    CUDA_TRY(cudaMalloc(&d, cap * sizeof(XgmWorkItem)));
-    have = cap;
-    return XGM_OK;
-}
-
-static xgm_status ensure_levels(xgm_searcher* s, size_t need, int which) {
-    if (need <= s->levels_cap[which]) return XGM_OK;
-    size_t cap = std::max<size_t>(need * 2, 1024);
-    CUDA_TRY(cudaStreamSynchronize(s->stream));
-    if (s->h_levels[which]) cudaFreeHost(s->h_levels[which]);
-    cudaFree(s->d_levels[which]);
-    s->h_levels[which] = nullptr; s->d_levels[which] = nullptr;
-    CUDA_TRY(cudaMallocHost(&s->h_levels[which], cap * 4));
-    CUDA_TRY(cudaMalloc(&s->d_levels[which], cap * 4));
-    s->levels_cap[which] = cap;
-    return XGM_OK;
-}
-
-static xgm_status ensure_expanded(xgm_searcher* s, size_t need, int which) {
-    if (need <= s->exp_cap[which]) return XGM_OK;
-    size_t cap = std::max<size_t>(need * 2, 65536);
-    CUDA_TRY(cudaStreamSynchronize(s->stream));
-    cudaFree(s->d_exp[which]);
-    s->d_exp[which] = nullptr;
-    CUDA_TRY(cudaMalloc(&s->d_exp[which], cap * sizeof(XgmWorkItem)));
-    s->exp_cap[which] = cap;
-    return XGM_OK;
 }
 
 extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, uint32_t max_topk, xgm_searcher** out) {
@@ -1123,10 +1140,10 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
     }
     if (const char* e = getenv("XGM_SHARED_COMPUTE")) s->shared_compute = atoi(e) != 0;
     if (const char* e = getenv("XGM_RANGE_BITS")) s->range_bits = (uint32_t)std::min(31, std::max(0, atoi(e)));
-    CUDA_TRY(cudaMalloc(&s->d_rng_total, 64));
-    CUDA_TRY(cudaMemset(s->d_rng_total, 0, 64));
-    CUDA_TRY(cudaMallocHost(&s->h_rng_total, 64));
-    s->h_rng_total[0] = 0;
+    CUDA_TRY(cudaMalloc(&s->bm_list.d_rng_total, 64));
+    CUDA_TRY(cudaMemset(s->bm_list.d_rng_total, 0, 64));
+    CUDA_TRY(cudaMallocHost(&s->bm_list.h_rng_total, 64));
+    s->bm_list.h_rng_total[0] = 0;
     {
         std::lock_guard<std::mutex> lk(ix->launch_mu);
         if (!ix->compute_stream) CUDA_TRY(cudaStreamCreateWithFlags(&ix->compute_stream, cudaStreamNonBlocking));
@@ -1163,11 +1180,9 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
     if (const char* e = getenv("XGM_POOL_ENTRIES")) s->pool_total = (uint32_t)strtoul(e, nullptr, 10);
     CUDA_TRY(cudaMalloc(&s->d_pool_w, (size_t)s->pool_total * 8)); CUDA_TRY(cudaMalloc(&s->d_pool_d, (size_t)s->pool_total * 4));
     CUDA_TRY(cudaMalloc(&s->d_pool_k, (size_t)s->pool_total * 8));
-    xgm_status st = ensure_items(s.get(), 4096, 0);
-    if (st != XGM_OK) return st;
-    st = ensure_items(s.get(), 4096, 1);
-    if (st != XGM_OK) return st;
-    st = ensure_items(s.get(), 4096, 2);
+    xgm_status st = s->and_list.seg.reserve(4096, 4096, s->stream);
+    if (st == XGM_OK) st = s->or_list.seg.reserve(4096, 4096, s->stream);
+    if (st == XGM_OK) st = s->bm_list.seg.reserve(4096, 4096, s->stream);
     if (st != XGM_OK) return st;
     int occ = xgm_and_occupancy_blocks_per_sm();
     if (occ < 1) occ = 1;
@@ -1184,10 +1199,6 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
     occ = xgm_and_bm_occupancy_blocks_per_sm();
     if (occ < 1) occ = 1;
     s->grid_bm = ix->sm_count * occ;
-    occ = xgm_and2_occupancy_blocks_per_sm();
-    if (occ < 1) occ = 1;
-    s->grid_and2 = ix->sm_count * occ;
-    if (const char* e = getenv("XGM_AND_KERNEL")) s->and_version = atoi(e) == 2 ? 2 : 1;
     *out = s.release();
     return XGM_OK;
 }
@@ -1298,8 +1309,7 @@ static double bm25_maxpart(double termweight, double len_factor, double k1, doub
 }
 
 static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, PlannedQuery& pq, XgmDevQuery& dq,
-                             std::vector<XgmWorkItem>& items, std::vector<XgmWorkItem>& items_or,
-                             std::vector<XgmWorkItem>& items_bm, uint32_t blocks_per_item) {
+                             PlannedSegments& segs) {
     const xgm_index* ix = s->ix;
     pq = PlannedQuery();
     memset(&dq, 0, offsetof(XgmDevQuery, terms)); /* the term slots in use are written in full by put_term */
@@ -1308,10 +1318,10 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
     const uint32_t nfilter = q.nfilter, nnot = q.nnot, nmaybe = q.nmaybe, ngroups = q.nfilter + q.nnot + q.nmaybe;
     if (ngroups) {
         /* OP_FILTER with boolean terms / OP_AND_NOT / OP_AND_MAYBE around an AND (or single-term) base, the first
-         * two also around an OR base; optional leaves on an OR base, a value-range filter on top, or the chunked
-         * kernel variant are left to the reference */
+         * two also around an OR base; optional leaves on an OR base or a value-range filter on top are left to the
+         * reference */
         const bool or_base = q.op == XGM_OP_OR && q.nterms != 1;
-        if ((or_base && q.nmaybe) || q.filter != XGM_FILTER_NONE || s->and_version != 1 ||
+        if ((or_base && q.nmaybe) || q.filter != XGM_FILTER_NONE ||
             (uint64_t)q.nterms + ngroups > XGM_MAX_TERMS) {
             pq.status = XGM_E_UNIMPLEMENTED;
             return XGM_OK;
@@ -1329,7 +1339,7 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
      * termfreq (min, est, max) = (0, value_freq, value_freq) (range.cc:457-464, api/postingsource.cc:201-214) */
     const bool mv_source = q.filter == XGM_FILTER_MULTI_RANGE;
     const bool src_weighted = mv_source && q.filter_weighted;
-    if (q.filter_weighted && (!mv_source || (q.op != XGM_OP_AND && q.nterms != 1) || ngroups || s->and_version != 1)) { pq.status = XGM_E_UNIMPLEMENTED; return XGM_OK; }
+    if (q.filter_weighted && (!mv_source || (q.op != XGM_OP_AND && q.nterms != 1) || ngroups)) { pq.status = XGM_E_UNIMPLEMENTED; return XGM_OK; }
     const double src_w = src_weighted ? (q.filter_factor != 0.0 ? q.filter_factor : 1.0) * 1.0 : 0.0;
     if (src_w < 0.0) { pq.status = XGM_E_UNIMPLEMENTED; return XGM_OK; }
     const uint32_t n = q.nterms;
@@ -1671,12 +1681,11 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
     if (dq.route == 1 && group_absent) { pq.on_device = false; return XGM_OK; } /* OR filtered by an absent term: empty */
     pq.on_device = true;
     /* one segment per (query[, leaf]); the device expands segments into work items (xgm_expand_items_kernel) */
-    (void)blocks_per_item;
     if (dq.route == 0) {
         /* every list but the driver has a membership bitmap → lean bitmap kernel */
-        bool all_bm = dq.nterms >= 2 && s->and_version == 1;
+        bool all_bm = dq.nterms >= 2;
         for (uint32_t i = 1; i < dq.nterms + dq.nnot; ++i) all_bm = all_bm && dq.terms[i].bm_off != XGM_NO_BITMAP;
-        std::vector<XgmWorkItem>& dst = all_bm ? items_bm : items;
+        std::vector<XgmWorkItem>& dst = all_bm ? segs.bm_list : segs.and_list;
         XgmWorkItem wi;
         wi.query = qi; wi.b0 = dq.terms[0].nblocks; wi.b1 = 0; wi.pad = 0;
         if (wi.b0) dst.push_back(wi);
@@ -1688,10 +1697,155 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
         for (uint32_t leaf = 0; leaf < n; ++leaf) {
             XgmWorkItem wi;
             wi.query = qi; wi.b0 = dq.terms[leaf].nblocks; wi.b1 = 0; wi.pad = leaf;
-            if (wi.b0) items_or.push_back(wi);
+            if (wi.b0) segs.or_list.push_back(wi);
         }
     }
     return XGM_OK;
+}
+
+/* Level starts of segments sorted by descending length: level k holds the k-th item of every segment that has one,
+ * i.e. a prefix of the sorted segments.  Writes the nlev + 1 starts to lv and returns the number of items. */
+static uint64_t level_starts(const XgmWorkItem* v, size_t n, uint32_t nlev, uint32_t bpi, uint32_t* lv) {
+    uint64_t run = 0;
+    size_t alive = n;
+    for (uint32_t k = 0; k < nlev; ++k) {
+        while (alive > 0 && (v[alive - 1].b0 + bpi - 1) / bpi <= k) --alive;
+        lv[k] = (uint32_t)run;
+        run += alive;
+    }
+    lv[nlev] = (uint32_t)run;
+    return run;
+}
+
+/* Level order: the general AND list, and the bitmap AND list of batches under 256 queries */
+static xgm_status order_levels(WorkList& L, std::vector<XgmWorkItem>& v, uint32_t bpi, cudaStream_t st) {
+    xgm_status r = L.seg.reserve(v.size(), 4096, st);
+    if (r != XGM_OK) return r;
+    uint64_t run = 0;
+    L.nstarts = 0;
+    if (!v.empty()) {
+        std::sort(v.begin(), v.end(), [](const XgmWorkItem& a, const XgmWorkItem& b) { return a.b0 > b.b0; });
+        const uint32_t maxlev = (v[0].b0 + bpi - 1) / bpi;
+        r = L.levels.reserve((size_t)maxlev + 1, 1024, st);
+        if (r != XGM_OK) return r;
+        run = level_starts(v.data(), v.size(), maxlev, bpi, L.levels.h);
+        L.nstarts = maxlev + 1;
+        std::copy(v.begin(), v.end(), L.seg.h);
+    }
+    L.nseg = (uint32_t)v.size();
+    return L.set_items(run, st);
+}
+
+/* OR list: leaf-major groups (all queries' rarest leaves first: by the time the frequent, low-weight leaves come up
+ * the thresholds have risen and MaxScore skips them wholesale), level order inside each group so that one query's
+ * items are spread in time and its threshold settles early */
+static xgm_status order_or_groups(OrList& L, std::vector<XgmWorkItem>& v, uint32_t bpi, cudaStream_t st) {
+    xgm_status r = L.seg.reserve(v.size(), 4096, st);
+    if (r != XGM_OK) return r;
+    std::stable_sort(v.begin(), v.end(), [](const XgmWorkItem& a, const XgmWorkItem& b) { return a.pad < b.pad; });
+    size_t nstarts = 0;
+    for (size_t a = 0; a < v.size();) {
+        size_t b = a;
+        while (b < v.size() && v[b].pad == v[a].pad) ++b;
+        std::sort(v.begin() + a, v.begin() + b, [](const XgmWorkItem& x, const XgmWorkItem& y) { return x.b0 > y.b0; });
+        nstarts += (v[a].b0 + bpi - 1) / bpi + 1;
+        a = b;
+    }
+    r = L.levels.reserve(nstarts, 1024, st);
+    if (r != XGM_OK) return r;
+    L.groups.clear();
+    uint64_t run = 0;
+    size_t lvpos = 0;
+    for (size_t a = 0; a < v.size();) {
+        size_t b = a;
+        while (b < v.size() && v[b].pad == v[a].pad) ++b;
+        OrList::Group g;
+        g.seg_off = (uint32_t)a; g.nseg = (uint32_t)(b - a); g.level_off = (uint32_t)lvpos;
+        g.nlevels = (v[a].b0 + bpi - 1) / bpi;
+        g.out_off = (uint32_t)run;
+        const uint64_t n = level_starts(v.data() + a, b - a, g.nlevels, bpi, L.levels.h + lvpos);
+        g.total = (uint32_t)n;
+        run += n;
+        lvpos += (size_t)g.nlevels + 1;
+        L.groups.push_back(g);
+        a = b;
+    }
+    std::copy(v.begin(), v.end(), L.seg.h);
+    L.nseg = (uint32_t)v.size();
+    L.nstarts = (uint32_t)lvpos;
+    return L.set_items(run, st);
+}
+
+/* Range-major order of the bitmap AND list (batches of 256 queries or more), expanded on the device
+ * (xgm_range_*_kernel).  Segments sorted by driver list (terms[0]), ties by query index.  Up to XGM_BM_RUN
+ * consecutive segments with the same driver form a run, and the run's items serve all of its queries: the AND
+ * kernel decodes the driver's blocks once per range and probes them for each query.  The runs follow the segments
+ * in the upload as {first segment, #driver blocks, the driver's first header, #queries}.  The host only bounds the
+ * number of items: every range can add one partial item per run. */
+static xgm_status order_driver_runs(xgm_searcher* s, std::vector<XgmWorkItem>& v, uint32_t bpi) {
+    BmList& L = s->bm_list;
+    xgm_status r = L.seg.reserve(2 * v.size(), 4096, s->stream); /* segments, then at most as many runs */
+    if (r != XGM_OK) return r;
+    L.nranges = (s->ix->lastdocid >> s->range_bits) + 1;
+    const XgmDevQuery* hq = s->h_queries;
+    auto drv = [hq](const XgmWorkItem& a) { return hq[a.query].terms[0].blk_begin; };
+    std::sort(v.begin(), v.end(), [&](const XgmWorkItem& a, const XgmWorkItem& b) {
+        return drv(a) != drv(b) ? drv(a) < drv(b) : a.query < b.query;
+    });
+    XgmWorkItem* h = L.seg.h;
+    const size_t nseg = v.size();
+    uint64_t run = 0;
+    for (size_t i = 0; i < nseg; ++i) {
+        h[i] = v[i];
+        XgmWorkItem* last = h + nseg + L.nruns - 1;
+        if (L.nruns != 0 && last->b1 == drv(v[i]) && last->pad < XGM_BM_RUN) {
+            ++last->pad;
+            continue;
+        }
+        h[nseg + L.nruns++] = XgmWorkItem{(uint32_t)i, v[i].b0, drv(v[i]), 1u};
+        run += (v[i].b0 + bpi - 1) / bpi;
+    }
+    /* most work first within each range (queries x driver blocks), so that the batch does not end on a long item */
+    std::stable_sort(h + nseg, h + nseg + L.nruns, [](const XgmWorkItem& a, const XgmWorkItem& b) {
+        return (uint64_t)a.pad * a.b0 > (uint64_t)b.pad * b.b0;
+    });
+    run += (uint64_t)L.nruns * L.nranges;
+    const size_t need = (size_t)L.nranges * L.nruns * 3; /* first blocks, counts, offsets */
+    if (need > L.rng_cap) {
+        CUDA_TRY(cudaStreamSynchronize(s->stream));
+        if (s->ix->compute_stream) CUDA_TRY(cudaStreamSynchronize(s->ix->compute_stream));
+        cudaFree(L.d_rng);
+        L.d_rng = nullptr; L.rng_cap = 0;
+        CUDA_TRY(cudaMalloc(&L.d_rng, need * 2 * sizeof(uint32_t)));
+        L.rng_cap = need * 2;
+    }
+    L.nseg = (uint32_t)nseg;
+    L.nstarts = 0;
+    return L.set_items(run, s->stream);
+}
+
+static cudaError_t expand_levels(const WorkList& L, uint32_t bpi, cudaStream_t cs, uint32_t& launches) {
+    if (!L.nitems) return cudaSuccess;
+    ++launches;
+    return xgm_launch_expand(L.seg.d, L.nseg, L.nitems, L.levels.d, L.nstarts - 1, bpi, L.d_exp, cs);
+}
+
+static cudaError_t expand_or_groups(const OrList& L, uint32_t bpi, cudaStream_t cs, uint32_t& launches) {
+    for (const auto& g : L.groups) {
+        cudaError_t e = xgm_launch_expand(L.seg.d + g.seg_off, g.nseg, g.total, L.levels.d + g.level_off, g.nlevels, bpi,
+                                          L.d_exp + g.out_off, cs);
+        if (e != cudaSuccess) return e;
+        ++launches;
+    }
+    return cudaSuccess;
+}
+
+static cudaError_t expand_driver_runs(const BmList& L, const XgmBlockHdr* hdr, uint32_t range_bits, uint32_t bpi,
+                                      cudaStream_t cs, uint32_t& launches) {
+    const size_t n = (size_t)L.nranges * L.nruns;
+    launches += 3;
+    return xgm_launch_expand_ranges(L.seg.d + L.nseg, L.nruns, hdr, L.nranges, range_bits, bpi, L.d_rng, L.d_rng + n,
+                                    L.d_rng + 2 * n, L.d_rng_total, L.d_exp, cs);
 }
 
 static xgm_status launch_batch(xgm_searcher* s) {
@@ -1710,36 +1864,16 @@ static xgm_status launch_batch(xgm_searcher* s) {
     CUDA_TRY(cudaMemsetAsync(p.hist, 0, (size_t)s->nq * XGM_NBINS * 4, cs));
     s->stats.kernel_launches = 0;
     p.pass = 0;
-    {
-        const XgmWorkItem* segs[3] = {s->d_items, s->d_items_or, s->d_items_bm};
-        const uint32_t totals[3] = {s->nitems, s->nitems_or, s->nitems_bm};
-        for (int w = 0; w < 3; ++w) {
-            if (!totals[w]) continue;
-            if (w == 1) {
-                for (const auto& g : s->or_groups) {
-                    CUDA_TRY(xgm_launch_expand(segs[1] + g.seg_off, g.nseg, g.total, s->d_levels[1] + g.level_off, g.nlevels,
-                                               s->bpi, s->d_exp[1] + g.out_off, cs));
-                    s->stats.kernel_launches++;
-                }
-            } else if (w == 2 && s->range_mode) {
-                const size_t n = (size_t)s->nranges * s->nruns;
-                CUDA_TRY(xgm_launch_expand_ranges(segs[2] + s->nseg[2], s->nruns, p.hdr, s->nranges, s->range_bits, s->bpi,
-                                                  s->d_rng, s->d_rng + n, s->d_rng + 2 * n, s->d_rng_total, s->d_exp[2], cs));
-                s->stats.kernel_launches += 3;
-            } else {
-                CUDA_TRY(xgm_launch_expand(segs[w], s->nseg[w], totals[w], s->d_levels[w], s->nlevels[w], s->bpi, s->d_exp[w], cs));
-                s->stats.kernel_launches++;
-            }
-        }
-    }
+    uint32_t& launches = s->stats.kernel_launches;
+    CUDA_TRY(expand_levels(s->and_list, s->bpi, cs, launches));
+    CUDA_TRY(expand_or_groups(s->or_list, s->bpi, cs, launches));
+    CUDA_TRY(s->bm_list.range_mode ? expand_driver_runs(s->bm_list, p.hdr, s->range_bits, s->bpi, cs, launches)
+                                   : expand_levels(s->bm_list, s->bpi, cs, launches));
     CUDA_TRY(cudaEventRecord(s->ev0, cs));
-    auto launch_and = [&](const XgmKernelParams& pp) {
-        return s->and_version == 1 ? xgm_launch_and(pp, s->grid, cs) : xgm_launch_and2(pp, s->grid_and2, cs);
-    };
-    if (s->nitems_bm) { CUDA_TRY(xgm_launch_and_bm(p, s->grid_bm, cs)); s->stats.kernel_launches++; }
-    if (s->nitems) { CUDA_TRY(launch_and(p)); s->stats.kernel_launches++; }
-    if (s->nitems_or && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p, s->grid_or3, 0, cs)); s->stats.kernel_launches++; }
-    if (s->nitems_or && s->any_or_slow) { CUDA_TRY(xgm_launch_or(p, s->grid_or, cs)); s->stats.kernel_launches++; }
+    if (s->bm_list.nitems) { CUDA_TRY(xgm_launch_and_bm(p, s->grid_bm, cs)); s->stats.kernel_launches++; }
+    if (s->and_list.nitems) { CUDA_TRY(xgm_launch_and(p, s->grid, cs)); s->stats.kernel_launches++; }
+    if (s->or_list.nitems && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p, s->grid_or3, 0, cs)); s->stats.kernel_launches++; }
+    if (s->or_list.nitems && s->any_or_slow) { CUDA_TRY(xgm_launch_or(p, s->grid_or, cs)); s->stats.kernel_launches++; }
     if (s->ntileq) { /* documents with >= 2 leaves by bitmap union, then the single-leaf ones against the threshold */
         CUDA_TRY(xgm_launch_or_tile(p, s->grid_tile, cs));
         CUDA_TRY(xgm_launch_or3(p, s->grid_or3, 1, cs));
@@ -1751,10 +1885,10 @@ static xgm_status launch_batch(xgm_searcher* s) {
     /* second pass: only queries whose candidate buffer overflowed do any work (device-side flag) */
     XgmKernelParams p2 = p;
     p2.pass = 1;
-    if (s->nitems_bm) { CUDA_TRY(xgm_launch_and_bm(p2, s->grid_bm, cs)); s->stats.kernel_launches++; }
-    if (s->nitems) { CUDA_TRY(launch_and(p2)); s->stats.kernel_launches++; }
-    if (s->nitems_or && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p2, s->grid_or3, 0, cs)); s->stats.kernel_launches++; }
-    if (s->nitems_or && s->any_or_slow) { CUDA_TRY(xgm_launch_or(p2, s->grid_or, cs)); s->stats.kernel_launches++; }
+    if (s->bm_list.nitems) { CUDA_TRY(xgm_launch_and_bm(p2, s->grid_bm, cs)); s->stats.kernel_launches++; }
+    if (s->and_list.nitems) { CUDA_TRY(xgm_launch_and(p2, s->grid, cs)); s->stats.kernel_launches++; }
+    if (s->or_list.nitems && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p2, s->grid_or3, 0, cs)); s->stats.kernel_launches++; }
+    if (s->or_list.nitems && s->any_or_slow) { CUDA_TRY(xgm_launch_or(p2, s->grid_or, cs)); s->stats.kernel_launches++; }
     if (s->ntileq) {
         CUDA_TRY(xgm_launch_or_tile(p2, s->grid_tile, cs));
         CUDA_TRY(xgm_launch_or3(p2, s->grid_or3, 1, cs));
@@ -1776,187 +1910,68 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     CUDA_TRY(cudaSetDevice(s->ix->device));
     s->plan.resize(nq);
     s->nq = nq;
-    /* work granularity: enough items to balance ~grid*8 warps, at most 32 driver blocks per item */
-    uint64_t total_drv_blocks = 0;
-    std::vector<XgmWorkItem> items, items_or, items_bm;
-    items.reserve(4096);
-    /* first pass with a provisional granularity needs the driver block counts; plan twice is wasteful,
-     * so use a fixed small granularity scaled by batch size */
+    PlannedSegments segs;
+    segs.and_list.reserve(4096);
+    /* work granularity: enough items to balance ~grid*8 warps, at most 32 driver blocks per item.  Finding it from
+     * the driver block counts would mean planning twice, so it is a fixed small granularity scaled by batch size. */
     uint32_t bpi = nq >= 256 ? 12 : (nq >= 16 ? 4 : 1); /* 12: scripts/sweep_bm.py, 8..32 x range widths 2^17..2^20 */
-    if (s->and_version == 2) bpi = nq >= 64 ? 16 : (nq >= 8 ? 8 : 4);
     if (s->bpi_override && nq >= 256) bpi = s->bpi_override; /* XGM_BPI: measurement aid */
     s->any_sort = false;
-    uint64_t alg = 0, postings = 0;
+    uint64_t alg = 0;
     /* Planning (term lookup, Weight::init_, evaluation order, work items) is independent per query:
      * large batches are planned by a few host threads, each into its own work lists. */
     int T = 1;
     if (nq >= 512) T = PlannerPool::get().threads();
     if (T <= 1) {
         for (uint32_t i = 0; i < nq; ++i) {
-            xgm_status st = plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], items, items_or, items_bm, bpi);
+            xgm_status st = plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], segs);
             if (st != XGM_OK) return st;
         }
     } else {
-        std::vector<std::vector<XgmWorkItem>> ti(T), tio(T), tib(T);
+        std::vector<PlannedSegments> ts(T);
         std::vector<xgm_status> tst(T, XGM_OK);
         PlannerPool::get().run(T, [&](int t) {
             uint32_t a = (uint32_t)((uint64_t)nq * t / T), b = (uint32_t)((uint64_t)nq * (t + 1) / T);
-            tib[t].reserve((size_t)(b - a));
+            ts[t].bm_list.reserve((size_t)(b - a));
             for (uint32_t i = a; i < b; ++i) {
-                xgm_status st = plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], ti[t], tio[t], tib[t], bpi);
+                xgm_status st = plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], ts[t]);
                 if (st != XGM_OK) { tst[t] = st; return; }
             }
         });
         for (int t = 0; t < T; ++t) {
             if (tst[t] != XGM_OK) return fail(tst[t], "query planning failed");
-            items.insert(items.end(), ti[t].begin(), ti[t].end());
-            items_or.insert(items_or.end(), tio[t].begin(), tio[t].end());
-            items_bm.insert(items_bm.end(), tib[t].begin(), tib[t].end());
+            segs.and_list.insert(segs.and_list.end(), ts[t].and_list.begin(), ts[t].and_list.end());
+            segs.or_list.insert(segs.or_list.end(), ts[t].or_list.begin(), ts[t].or_list.end());
+            segs.bm_list.insert(segs.bm_list.end(), ts[t].bm_list.begin(), ts[t].bm_list.end());
         }
     }
     const auto t_planned = std::chrono::steady_clock::now();
     for (uint32_t i = 0; i < nq; ++i) {
         if (s->plan[i].sort_by || s->h_queries[i].route == 1 || s->plan[i].aux_subqs) s->any_sort = true; /* keys/aux needed on the host */
         alg += s->plan[i].alg_bytes;
-        total_drv_blocks += s->h_queries[i].terms[0].nblocks;
     }
-    (void)total_drv_blocks; (void)postings;
-    /* OR work is ordered leaf-major (all queries' rarest leaves first): by the time the frequent, low-weight
-     * leaves come up the thresholds have risen and MaxScore skips them wholesale */
-    std::stable_sort(items_or.begin(), items_or.end(),
-                     [](const XgmWorkItem& a, const XgmWorkItem& b) { return a.pad < b.pad; });
-    /* segments → pinned staging with the running item index; totals and permutation strides */
-    xgm_status st = XGM_OK;
+    /* segments → each list's pinned staging, in the order the device expands them */
     s->bpi = bpi;
-    {
-        std::vector<XgmWorkItem>* lists[3] = {&items, &items_or, &items_bm};
-        XgmWorkItem** hbuf[3] = {&s->h_items, &s->h_items_or, &s->h_items_bm};
-        uint32_t* totals[3] = {&s->nitems, &s->nitems_or, &s->nitems_bm};
-        for (int w = 0; w < 3; ++w) {
-            std::vector<XgmWorkItem>& v = *lists[w];
-            st = ensure_items(s, w == 2 ? 2 * v.size() : v.size(), w); /* the bitmap list may add its runs */
-            if (st != XGM_OK) return st;
-            uint64_t run = 0;
-            XgmWorkItem* h = *hbuf[w];
-            s->nlevels[w] = 0;
-            if (w == 2) { s->range_mode = false; s->nruns = 0; }
-            if (w == 2 && !v.empty() && nq >= 256 && s->range_bits != 0) {
-                /* range-major order, expanded on the device (xgm_range_*_kernel): the host only bounds the
-                 * number of items — every range can add one partial item per run */
-                s->range_mode = true;
-                s->nranges = (s->ix->lastdocid >> s->range_bits) + 1;
-                /* Segments sorted by driver list (terms[0]), ties by query index.  Up to XGM_BM_RUN consecutive segments
-                 * with the same driver form a run, and the run's items serve all of its queries: the AND kernel decodes
-                 * the driver's blocks once per range and probes them for each query.  The runs follow the segments in
-                 * the upload as {first segment, #driver blocks, the driver's first header, #queries}. */
-                const XgmDevQuery* hq = s->h_queries;
-                auto drv = [hq](const XgmWorkItem& a) { return hq[a.query].terms[0].blk_begin; };
-                std::sort(v.begin(), v.end(), [&](const XgmWorkItem& a, const XgmWorkItem& b) {
-                    return drv(a) != drv(b) ? drv(a) < drv(b) : a.query < b.query;
-                });
-                const size_t nseg = v.size();
-                for (size_t i = 0; i < nseg; ++i) {
-                    h[i] = v[i];
-                    XgmWorkItem* last = h + nseg + s->nruns - 1;
-                    if (s->nruns != 0 && last->b1 == drv(v[i]) && last->pad < XGM_BM_RUN) {
-                        ++last->pad;
-                        continue;
-                    }
-                    h[nseg + s->nruns++] = XgmWorkItem{(uint32_t)i, v[i].b0, drv(v[i]), 1u};
-                    run += (v[i].b0 + bpi - 1) / bpi;
-                }
-                /* most work first within each range (queries x driver blocks), so that the batch does not end on a
-                 * long item */
-                std::stable_sort(h + nseg, h + nseg + s->nruns, [](const XgmWorkItem& a, const XgmWorkItem& b) {
-                    return (uint64_t)a.pad * a.b0 > (uint64_t)b.pad * b.b0;
-                });
-                run += (uint64_t)s->nruns * s->nranges; /* every range can add one partial item per run */
-                const size_t need = (size_t)s->nranges * s->nruns * 3; /* first blocks, counts, offsets */
-                if (need > s->rng_cap) {
-                    CUDA_TRY(cudaStreamSynchronize(s->stream));
-                    if (s->ix->compute_stream) CUDA_TRY(cudaStreamSynchronize(s->ix->compute_stream));
-                    cudaFree(s->d_rng);
-                    s->d_rng = nullptr;
-                    CUDA_TRY(cudaMalloc(&s->d_rng, need * 2 * sizeof(uint32_t)));
-                    s->rng_cap = need * 2;
-                }
-            } else if (w != 1 && !v.empty()) {
-                /* AND lists: level order — sort segments by descending length, level k holds the k-th item of
-                 * every segment that has one, i.e. a prefix of the sorted segments */
-                std::sort(v.begin(), v.end(), [](const XgmWorkItem& a, const XgmWorkItem& b) { return a.b0 > b.b0; });
-                const uint32_t maxlev = (v[0].b0 + bpi - 1) / bpi;
-                st = ensure_levels(s, (size_t)maxlev + 1, w);
-                if (st != XGM_OK) return st;
-                uint32_t* lv = s->h_levels[w];
-                size_t alive = v.size();
-                for (uint32_t k = 0; k < maxlev; ++k) {
-                    while (alive > 0 && (v[alive - 1].b0 + bpi - 1) / bpi <= k) --alive;
-                    lv[k] = (uint32_t)run;
-                    run += alive;
-                }
-                lv[maxlev] = (uint32_t)run;
-                s->nlevels[w] = maxlev;
-                for (size_t i = 0; i < v.size(); ++i) h[i] = v[i];
-            } else if (w == 1) {
-                /* OR: leaf-major groups (rarest leaves of all queries first, for MaxScore), level order inside
-                 * each group so that one query's items are spread in time and its threshold settles early */
-                s->or_groups.clear();
-                size_t nlev_total = 0;
-                for (size_t a = 0; a < v.size();) {
-                    size_t b = a;
-                    while (b < v.size() && v[b].pad == v[a].pad) ++b;
-                    std::sort(v.begin() + a, v.begin() + b, [](const XgmWorkItem& x, const XgmWorkItem& y) { return x.b0 > y.b0; });
-                    nlev_total += (v[a].b0 + bpi - 1) / bpi + 1;
-                    a = b;
-                }
-                st = ensure_levels(s, nlev_total + 1, 1);
-                if (st != XGM_OK) return st;
-                uint32_t* lv = s->h_levels[1];
-                size_t lvpos = 0;
-                for (size_t a = 0; a < v.size();) {
-                    size_t b = a;
-                    while (b < v.size() && v[b].pad == v[a].pad) ++b;
-                    const uint32_t maxlev = (v[a].b0 + bpi - 1) / bpi;
-                    xgm_searcher::OrGroup g;
-                    g.seg_off = (uint32_t)a; g.nseg = (uint32_t)(b - a); g.level_off = (uint32_t)lvpos; g.nlevels = maxlev;
-                    g.out_off = (uint32_t)run;
-                    uint64_t grun = 0;
-                    size_t alive = b - a;
-                    for (uint32_t k = 0; k < maxlev; ++k) {
-                        while (alive > 0 && (v[a + alive - 1].b0 + bpi - 1) / bpi <= k) --alive;
-                        lv[lvpos + k] = (uint32_t)grun;
-                        grun += alive;
-                    }
-                    lv[lvpos + maxlev] = (uint32_t)grun;
-                    lvpos += (size_t)maxlev + 1;
-                    g.total = (uint32_t)grun;
-                    run += grun;
-                    s->or_groups.push_back(g);
-                    a = b;
-                }
-                s->nlevels[1] = (uint32_t)lvpos; /* total entries to copy */
-                for (size_t i = 0; i < v.size(); ++i) h[i] = v[i];
-            }
-            if (run >= 0xffffffffull) return fail(XGM_E_INVALID, "too many work items in one batch");
-            *totals[w] = (uint32_t)run;
-            s->nseg[w] = (uint32_t)v.size();
-            st = ensure_expanded(s, run, w);
-            if (st != XGM_OK) return st;
-        }
-    }
+    BmList& bm = s->bm_list;
+    bm.range_mode = !segs.bm_list.empty() && nq >= 256 && s->range_bits != 0;
+    bm.nruns = 0;
+    xgm_status st = order_levels(s->and_list, segs.and_list, bpi, s->stream);
+    if (st == XGM_OK) st = order_or_groups(s->or_list, segs.or_list, bpi, s->stream);
+    if (st == XGM_OK) st = bm.range_mode ? order_driver_runs(s, segs.bm_list, bpi) : order_levels(bm, segs.bm_list, bpi, s->stream);
+    if (st != XGM_OK) return st;
     const auto t_interleaved = std::chrono::steady_clock::now();
     s->stats = xgm_batch_stats{};
     s->stats.algorithmic_bytes = alg;
-    s->stats.work_items = s->nitems + s->nitems_or + s->nitems_bm;
-    s->stats.h2d_bytes = (uint64_t)nq * sizeof(XgmDevQuery) + (uint64_t)(s->nseg[0] + s->nseg[1] + s->nseg[2] + s->nruns) * sizeof(XgmWorkItem);
+    s->stats.work_items = s->and_list.nitems + s->or_list.nitems + bm.nitems;
+    s->stats.h2d_bytes = (uint64_t)nq * sizeof(XgmDevQuery) + (uint64_t)(s->and_list.nseg + s->or_list.nseg + bm.nseg + bm.nruns) * sizeof(XgmWorkItem);
     s->stats.d2h_bytes = (uint64_t)nq * sizeof(XgmDevResult) + (uint64_t)nq * s->max_topk * (8 + 4 + (s->any_sort ? 8 : 0));
     XgmKernelParams& p = s->params;
     fill_index_params(s->ix, p);
-    p.queries = s->d_queries; p.items = s->d_exp[0]; p.nitems = s->nitems; p.nq = nq;
-    p.items_or = s->d_exp[1]; p.nitems_or = s->nitems_or;
-    p.items_bm = s->d_exp[2]; p.nitems_bm = s->nitems_bm;
-    p.nitems_bm_dev = s->range_mode ? s->d_rng_total : nullptr;
-    p.bm_segs = s->range_mode ? s->d_items_bm : nullptr;
+    p.queries = s->d_queries; p.items = s->and_list.d_exp; p.nitems = s->and_list.nitems; p.nq = nq;
+    p.items_or = s->or_list.d_exp; p.nitems_or = s->or_list.nitems;
+    p.items_bm = bm.d_exp; p.nitems_bm = bm.nitems;
+    p.nitems_bm_dev = bm.range_mode ? bm.d_rng_total : nullptr;
+    p.bm_segs = bm.range_mode ? bm.seg.d : nullptr;
     p.work_counter = reinterpret_cast<uint32_t*>(s->d_ctrl);
     p.qstate = reinterpret_cast<XgmQState*>(s->d_ctrl + XGM_CTRL_HDR);
     p.hist = reinterpret_cast<uint32_t*>(s->d_ctrl + XGM_CTRL_HDR + (size_t)s->max_batch * sizeof(XgmQState));
@@ -1979,16 +1994,9 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     p.tileq = s->d_tileq; p.ntileq = s->ntileq;
     if (s->ntileq) CUDA_TRY(cudaMemcpyAsync(s->d_tileq, s->h_tileq, (size_t)s->ntileq * 4, cudaMemcpyHostToDevice, s->stream));
     CUDA_TRY(cudaMemcpyAsync(s->d_queries, s->h_queries, (size_t)nq * sizeof(XgmDevQuery), cudaMemcpyHostToDevice, s->stream));
-    if (s->nseg[0])
-        CUDA_TRY(cudaMemcpyAsync(s->d_items, s->h_items, (size_t)s->nseg[0] * sizeof(XgmWorkItem), cudaMemcpyHostToDevice, s->stream));
-    if (s->nseg[1])
-        CUDA_TRY(cudaMemcpyAsync(s->d_items_or, s->h_items_or, (size_t)s->nseg[1] * sizeof(XgmWorkItem), cudaMemcpyHostToDevice, s->stream));
-    if (s->nseg[2])
-        CUDA_TRY(cudaMemcpyAsync(s->d_items_bm, s->h_items_bm, (size_t)(s->nseg[2] + s->nruns) * sizeof(XgmWorkItem),
-                                 cudaMemcpyHostToDevice, s->stream));
-    for (int w = 0; w < 3; ++w)
-        if (s->nlevels[w])
-            CUDA_TRY(cudaMemcpyAsync(s->d_levels[w], s->h_levels[w], ((size_t)s->nlevels[w] + 1) * 4, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(s->and_list.upload(0, s->stream));
+    CUDA_TRY(s->or_list.upload(0, s->stream));
+    CUDA_TRY(bm.upload(bm.nruns, s->stream)); /* the runs follow the segments */
     if (g_trace) { s->tr_submit = t_submit0; s->tr_planned = t_interleaved; CUDA_TRY(cudaEventRecord(s->tr_h2d, s->stream)); }
     st = launch_batch(s);
     if (st != XGM_OK) return st;
@@ -2000,7 +2008,7 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
         return XGM_OK;
     }
     CUDA_TRY(cudaMemcpyAsync(s->h_info, s->d_info, (size_t)nq * sizeof(XgmDevResult), cudaMemcpyDeviceToHost, s->stream));
-    if (s->range_mode) CUDA_TRY(cudaMemcpyAsync(s->h_rng_total, s->d_rng_total, 4, cudaMemcpyDeviceToHost, s->stream));
+    if (bm.range_mode) CUDA_TRY(cudaMemcpyAsync(bm.h_rng_total, bm.d_rng_total, 4, cudaMemcpyDeviceToHost, s->stream));
     CUDA_TRY(cudaMemcpyAsync(s->h_out_w, s->d_out_w, ns * 8, cudaMemcpyDeviceToHost, s->stream));
     CUDA_TRY(cudaMemcpyAsync(s->h_out_d, s->d_out_d, ns * 4, cudaMemcpyDeviceToHost, s->stream));
     if (s->any_sort) CUDA_TRY(cudaMemcpyAsync(s->h_out_k, s->d_out_k, ns * 8, cudaMemcpyDeviceToHost, s->stream));
@@ -2016,7 +2024,7 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
                 std::chrono::duration<float, std::milli>(t_planned - t_submit0).count(),
                 std::chrono::duration<float, std::milli>(t_interleaved - t_planned).count(),
                 std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_interleaved).count(), T,
-                (size_t)s->nitems + s->nitems_or + s->nitems_bm);
+                (size_t)s->and_list.nitems + s->or_list.nitems + bm.nitems);
     return XGM_OK;
 }
 
@@ -2182,7 +2190,7 @@ extern "C" xgm_status xgm_search_wait(xgm_searcher* s, uint32_t* docids, double*
     cudaEventElapsedTime(&s->stats.match_kernel_ms, s->ev0, s->ev1);
     cudaEventElapsedTime(&s->stats.topk_kernel_ms, s->ev1, s->ev2);
     const auto t_wait0 = std::chrono::steady_clock::now();
-    if (s->range_mode) s->stats.work_items = (uint64_t)s->nitems + s->nitems_or + s->h_rng_total[0];
+    if (s->bm_list.range_mode) s->stats.work_items = (uint64_t)s->and_list.nitems + s->or_list.nitems + s->bm_list.h_rng_total[0];
     s->stats.second_pass_queries = 0;
     for (uint32_t i = 0; i < s->nq; ++i) {
         const PlannedQuery& pq = s->plan[i];

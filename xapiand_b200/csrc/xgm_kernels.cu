@@ -15,7 +15,6 @@
  */
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "xgm_device.h"
 
@@ -25,7 +24,7 @@
  * GPUs through the C-ABI (an xgm_index carries its device): remember the opted-in size per (kernel, device). */
 #define XGM_MAX_DEVICES 64
 static cudaError_t optin_smem(const void* fn, int which, size_t bytes) {
-    static size_t have[4][XGM_MAX_DEVICES]; /* raised monotonically; racing threads set the same or a larger value */
+    static size_t have[2][XGM_MAX_DEVICES]; /* raised monotonically; racing threads set the same or a larger value */
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
@@ -951,8 +950,7 @@ __device__ __forceinline__ void emit_match_lanes(const XgmKernelParams& p, uint3
  * path: score 32 matches (stage 2 full, or out of work) → finish 32 candidates (stage 1 full, or the item
  * ended) → fetch the next work item → probe the decoded pair of driver blocks for the next query slot of the
  * item's run → decode the next pair.  A pair is decoded once and probed once per query of the run. */
-template <int MINB>
-__global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const __grid_constant__ XgmKernelParams p) {
+__global__ void __launch_bounds__(BM3_WARPS * 32, 4) xgm_and_bm3_kernel(const __grid_constant__ XgmKernelParams p) {
     extern __shared__ __align__(16) unsigned char bm3_raw[];
     Bm3Scratch* scratch = reinterpret_cast<Bm3Scratch*>(bm3_raw);
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
@@ -1185,23 +1183,8 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, MINB) xgm_and_bm3_kernel(const
     }
 }
 
-static int g_bm_variant = -1; /* XGM_BM_VARIANT: 33/34/35 = launch bounds for 3/4/5 CTAs per SM */
-static int bm_variant() {
-    if (g_bm_variant < 0) {
-        const char* e = getenv("XGM_BM_VARIANT");
-        g_bm_variant = e ? atoi(e) : 34;
-        if (g_bm_variant < 33 || g_bm_variant > 35) g_bm_variant = 34;
-    }
-    return g_bm_variant;
-}
-
-typedef void (*bm3_fn)(const XgmKernelParams);
-static bm3_fn bm3_kernel(int v) {
-    return v == 33 ? xgm_and_bm3_kernel<3> : v == 35 ? xgm_and_bm3_kernel<5> : xgm_and_bm3_kernel<4>;
-}
-
 cudaError_t xgm_launch_and_bm(const XgmKernelParams& p, int grid, cudaStream_t s) {
-    bm3_kernel(bm_variant())<<<grid, BM3_WARPS * 32, sizeof(Bm3Scratch) * BM3_WARPS, s>>>(p);
+    xgm_and_bm3_kernel<<<grid, BM3_WARPS * 32, sizeof(Bm3Scratch) * BM3_WARPS, s>>>(p);
     return cudaGetLastError();
 }
 
@@ -1209,352 +1192,9 @@ cudaError_t xgm_launch_and_bm(const XgmKernelParams& p, int grid, cudaStream_t s
  * call once per searcher, after cudaSetDevice). */
 int xgm_and_bm_occupancy_blocks_per_sm() {
     int n = 0;
-    const bm3_fn f = bm3_kernel(bm_variant());
     const size_t smem = sizeof(Bm3Scratch) * BM3_WARPS;
-    cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, f, BM3_WARPS * 32, smem);
-    return n;
-}
-
-/* ------------------------------------------------------------------ chunked AND kernel (v2) */
-
-/* Same contract as xgm_and_kernel, organised for memory-level parallelism (the warp-autonomous kernel
- * is bound by its chain of dependent global round trips, ~20 per driver block).  A CTA owns a chunk of
- * up to 16 driver blocks (2048 candidate docids).  The candidates go into a shared-memory hash set; the
- * blocks of the next list that overlap the chunk's docid span are then fetched with all their headers
- * in one coalesced read and four bulk copies in flight per warp, decoded by all warps at once, and
- * every decoded posting probes the hash set in O(1).  When the survivors are few compared with the
- * blocks in the span the kernel gallops per survivor instead (the leapfrog of
- * MultiAndPostList::find_next_match, multiandpostlist.cc:179-206).  Scoring is lazy: wdf / doc length
- * are only fetched for documents confirmed by the second list. */
-#define A2_WARPS 8
-#define A2_THREADS (A2_WARPS * 32)
-#define A2_MAXBLK 16
-#define A2_CAND (A2_MAXBLK * XGM_BLOCK)
-#define A2_BMWORDS 1024u /* 32768-bit membership filter over (docid mod 32768) */
-#define A2_STAGES 4
-
-struct __align__(16) A2Smem {
-    uint32_t stage[A2_WARPS][A2_STAGES][STAGE_WORDS];
-    uint64_t bar[A2_WARPS][A2_STAGES];
-    double acc[A2_CAND];
-    uint32_t cand[A2_CAND];   /* ascending docids: index = blk*128 + position in driver block blk */
-    uint32_t hitpos[A2_CAND]; /* (block - lo) << 7 | position, valid where `hit` is set */
-    uint32_t bm[A2_BMWORDS];
-    uint32_t alive[A2_CAND / 32];
-    uint32_t hit[A2_CAND / 32];
-    uint32_t lo[XGM_DEV_MAX_TERMS], hi[XGM_DEV_MAX_TERMS]; /* block span of list j covering the chunk */
-    uint32_t item;
-    uint32_t n_alive;
-};
-
-/* index of docid d in the chunk's ascending candidate array (n entries, padded with the sentinel), or -1 */
-__device__ __forceinline__ int a2_find(const A2Smem& s, uint32_t d) {
-    uint32_t pos = 0;
-#pragma unroll
-    for (uint32_t step = A2_CAND / 2; step >= 1; step >>= 1)
-        if (s.cand[pos + step - 1] < d) pos += step;
-    return s.cand[pos] == d ? (int)pos : -1;
-}
-
-__global__ void __launch_bounds__(A2_THREADS, 3) xgm_and2_kernel(XgmKernelParams p) {
-    extern __shared__ __align__(16) unsigned char a2_raw[];
-    A2Smem& s = *reinterpret_cast<A2Smem*>(a2_raw);
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    if (lane < A2_STAGES) mbar_init(&s.bar[warp][lane], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncthreads();
-    uint32_t phases = 0; /* bit b = parity of this warp's staging barrier b */
-    const XgmBlockHdr* __restrict__ hdr = p.hdr;
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + 4) == 0) return;
-
-    auto stage_issue = [&](uint32_t b, const uint4* col, uint32_t off16, uint32_t bits) {
-        __syncwarp();
-        if (bits != 0 && lane == 0) {
-            mbar_expect_tx(&s.bar[warp][b], bits * 16u);
-            bulk_g2s(s.stage[warp][b], col + off16, bits * 16u, &s.bar[warp][b]);
-        }
-    };
-    auto stage_wait = [&](uint32_t b, uint32_t bits) {
-        if (bits == 0) return;
-        mbar_wait(&s.bar[warp][b], (phases >> b) & 1u);
-        phases ^= 1u << b;
-    };
-
-    for (;;) {
-        __syncthreads();
-        if (tid == 0) s.item = atomicAdd(p.work_counter + 2 * p.pass, 1u);
-        __syncthreads();
-        const uint32_t item = s.item;
-        if (item >= p.nitems) break;
-        const XgmWorkItem wi = p.items[item];
-        if (p.pass != 0 && p.qstate[wi.query].rerun == 0) continue;
-        const XgmDevQuery* q = &p.queries[wi.query];
-        const uint32_t nterms = q->nterms;
-        const uint32_t nb = wi.b1 - wi.b0;
-        const uint32_t drv_begin = q->terms[0].blk_begin;
-        const double tw0 = q->terms[0].termweight;
-
-        /* ---- driver blocks: both headers, then both bulk copies, in flight before anything waits ---- */
-        const uint32_t blk0 = warp, blk1 = warp + A2_WARPS;
-        XgmBlockHdr dh0, dh1;
-        dh0.meta = dh1.meta = 0; dh0.first = dh1.first = 0; dh0.doc_off = dh1.doc_off = 0; dh0.tf_off = dh1.tf_off = 0;
-        if (blk0 < nb) { const uint4 h = __ldg(reinterpret_cast<const uint4*>(hdr + drv_begin + wi.b0 + blk0)); dh0.first = h.x; dh0.doc_off = h.y; dh0.tf_off = h.z; dh0.meta = h.w; }
-        if (blk1 < nb) { const uint4 h = __ldg(reinterpret_cast<const uint4*>(hdr + drv_begin + wi.b0 + blk1)); dh1.first = h.x; dh1.doc_off = h.y; dh1.tf_off = h.z; dh1.meta = h.w; }
-        const uint32_t cmin = __ldg(&hdr[drv_begin + wi.b0].first);
-        const uint32_t cmax = __ldg(&hdr[drv_begin + wi.b1].first) - 1u; /* sentinel after the last block */
-        if (blk0 < nb) {
-            stage_issue(0, p.docs, dh0.doc_off, XGM_HDR_DOC_BITS(dh0.meta));
-            if (nterms == 1) stage_issue(2, p.tfs, dh0.tf_off, XGM_HDR_TF_BITS(dh0.meta));
-        }
-        if (blk1 < nb) {
-            stage_issue(1, p.docs, dh1.doc_off, XGM_HDR_DOC_BITS(dh1.meta));
-            if (nterms == 1) stage_issue(3, p.tfs, dh1.tf_off, XGM_HDR_TF_BITS(dh1.meta));
-        }
-        for (uint32_t i = tid; i < A2_BMWORDS; i += A2_THREADS) s.bm[i] = 0u;
-        for (uint32_t i = nb * XGM_BLOCK + tid; i < A2_CAND; i += A2_THREADS) s.cand[i] = XGM_SENTINEL;
-        if (tid < A2_CAND / 32) { s.alive[tid] = 0u; s.hit[tid] = 0u; }
-        __syncthreads();
-
-        /* ---- spans of the other lists while the copies fly: one seek per (list, end) ---- */
-        for (uint32_t t = warp; t < 2 * (nterms - 1); t += A2_WARPS) {
-            const uint32_t j = 1 + (t >> 1);
-            if (q->terms[j].bm_off != XGM_NO_BITMAP) continue; /* probed through its bitmap: no span needed */
-            const XgmBlockHdr* lh = hdr + q->terms[j].blk_begin;
-            const uint32_t n = q->terms[j].nblocks;
-            XgmBlockHdr tmp;
-            uint32_t nf;
-            const uint32_t r = n ? warp_seek(lh, 0, n, (t & 1u) ? cmax : cmin, lane, tmp, nf) : 0u;
-            if (lane == 0) { if (t & 1u) s.hi[j] = r; else s.lo[j] = r; }
-        }
-
-#pragma unroll
-        for (int which = 0; which < 2; ++which) {
-            const uint32_t blk = which ? blk1 : blk0;
-            if (blk >= nb) continue;
-            const XgmBlockHdr dh = which ? dh1 : dh0;
-            const uint32_t dbits = XGM_HDR_DOC_BITS(dh.meta), dcount = XGM_HDR_COUNT(dh.meta);
-            const uint32_t tb = XGM_HDR_TF_BITS(dh.meta);
-            stage_wait(which, dbits);
-            uint32_t c[4];
-            decode_docids(s.stage[warp][which], dbits, dh.first, lane, c);
-            if (nterms == 1) stage_wait(2 + which, tb);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const bool valid = 4 * lane + k < dcount;
-                const uint32_t idx = blk * XGM_BLOCK + 4 * lane + k;
-                s.cand[idx] = valid ? c[k] : XGM_SENTINEL;
-                if (valid) {
-                    if (nterms == 1) {
-                        const uint32_t tf = tb ? unpack_sm(s.stage[warp][2 + which], 4 * lane + k, tb, bitmask(tb)) : 0u;
-                        s.acc[idx] = bm25_sumpart(tw0, q, tf, __ldg(&p.doclen[c[k]]));
-                    } else {
-                        atomicOr(&s.bm[(c[k] >> 5) & (A2_BMWORDS - 1)], 1u << (c[k] & 31));
-                    }
-                }
-            }
-            if (lane < 4) {
-                const uint32_t lo_pos = 32 * lane;
-                s.alive[blk * 4 + lane] = dcount >= lo_pos + 32 ? 0xffffffffu : (dcount > lo_pos ? ((1u << (dcount - lo_pos)) - 1u) : 0u);
-            }
-            __syncwarp();
-        }
-        __syncthreads();
-
-        /* ---- the other lists, ascending termfreq ---- */
-        for (uint32_t j = 1; j < nterms; ++j) {
-            if (warp == 0) {
-                uint32_t n = 0;
-                for (uint32_t w = lane; w < nb * 4; w += 32) n += __popc(s.alive[w]);
-                n = __reduce_add_sync(FULL, n);
-                if (lane == 0) s.n_alive = n;
-            }
-            __syncthreads();
-            const uint32_t n_alive = s.n_alive;
-            if (n_alive == 0) break;
-            const uint32_t lbegin = q->terms[j].blk_begin, lnblk = q->terms[j].nblocks;
-            const XgmBlockHdr* lh = hdr + lbegin;
-            const uint32_t lo = s.lo[j], hi = s.hi[j];
-            const double twj = q->terms[j].termweight;
-            const bool has_bm = q->terms[j].bm_off != XGM_NO_BITMAP;
-            if (has_bm) {
-                /* membership bitmap: one word load per surviving candidate, all in flight together;
-                 * 32 consecutive candidates belong to one warp, so the hit word is a ballot */
-                const uint32_t* __restrict__ bm = p.bitmaps + q->terms[j].bm_off;
-                for (uint32_t base = 0; base < nb * XGM_BLOCK; base += A2_THREADS) {
-                    const uint32_t idx = base + tid;
-                    const uint32_t aw = s.alive[idx >> 5];
-                    bool h = false;
-                    if (aw >> (idx & 31) & 1u) {
-                        const uint32_t d = s.cand[idx];
-                        h = (__ldg(bm + (d >> 5)) >> (d & 31)) & 1u;
-                    }
-                    const uint32_t bal = __ballot_sync(FULL, h);
-                    if (lane == 0) s.hit[idx >> 5] = bal;
-                }
-            } else if (lnblk != 0) {
-                const uint32_t nblk = hi - lo + 1;
-                if (nblk <= n_alive + 8) {
-                    /* dense: decode every block of the span.  A posting first tests the membership filter
-                     * (one shared-memory word), the few that pass binary-search the candidate array.
-                     * Per round a warp takes 32 blocks (lane i holds the header of its i-th block),
-                     * with A2_STAGES bulk copies in flight. */
-                    for (uint32_t base = lo; base <= hi; base += A2_WARPS * 32) {
-                        const uint32_t myb = base + warp + A2_WARPS * lane;
-                        uint4 hv = make_uint4(0u, 0u, 0u, 0u);
-                        if (myb <= hi) hv = __ldg(reinterpret_cast<const uint4*>(lh + myb));
-                        uint32_t cnt_w = 0;
-                        if (base + warp <= hi) cnt_w = (hi - (base + warp)) / A2_WARPS + 1;
-                        if (cnt_w > 32) cnt_w = 32;
-                        for (uint32_t i = 0; i < cnt_w && i < A2_STAGES; ++i) {
-                            const uint32_t off = __shfl_sync(FULL, hv.y, i), meta = __shfl_sync(FULL, hv.w, i);
-                            stage_issue(i, p.docs, off, XGM_HDR_DOC_BITS(meta));
-                        }
-                        for (uint32_t i = 0; i < cnt_w; ++i) {
-                            const uint32_t first = __shfl_sync(FULL, hv.x, i), meta = __shfl_sync(FULL, hv.w, i);
-                            const uint32_t bits = XGM_HDR_DOC_BITS(meta), cnt = XGM_HDR_COUNT(meta);
-                            const uint32_t sb = i % A2_STAGES;
-                            stage_wait(sb, bits);
-                            uint32_t bd[4];
-                            decode_docids(s.stage[warp][sb], bits, first, lane, bd);
-                            if (i + A2_STAGES < cnt_w) {
-                                const uint32_t off = __shfl_sync(FULL, hv.y, i + A2_STAGES);
-                                const uint32_t m2 = __shfl_sync(FULL, hv.w, i + A2_STAGES);
-                                stage_issue(sb, p.docs, off, XGM_HDR_DOC_BITS(m2));
-                            }
-                            const uint32_t brel = (base + warp + A2_WARPS * i) - lo;
-                            uint32_t flags = 0;
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                const uint32_t d = bd[k];
-                                if (4 * lane + k < cnt && d >= cmin && d <= cmax &&
-                                    (s.bm[(d >> 5) & (A2_BMWORDS - 1)] >> (d & 31) & 1u))
-                                    flags |= 1u << k;
-                            }
-                            while (__any_sync(FULL, flags != 0)) {
-                                if (flags) {
-                                    const int k = __ffs(flags) - 1;
-                                    flags &= flags - 1;
-                                    const uint32_t d = k == 0 ? bd[0] : k == 1 ? bd[1] : k == 2 ? bd[2] : bd[3];
-                                    const int idx = a2_find(s, d);
-                                    if (idx >= 0 && (s.alive[idx >> 5] >> (idx & 31) & 1u)) {
-                                        s.hitpos[idx] = (brel << 7) | (4 * lane + k);
-                                        atomicOr(&s.hit[idx >> 5], 1u << (idx & 31));
-                                    }
-                                }
-                            }
-                        }
-                    }
-                } else {
-                    /* sparse: gallop per surviving candidate */
-                    for (uint32_t w = warp; w < nb * 4; w += A2_WARPS) {
-                        uint32_t bits = s.alive[w];
-                        while (bits) {
-                            const uint32_t bit = __ffs(bits) - 1;
-                            bits &= bits - 1;
-                            const uint32_t idx = w * 32 + bit;
-                            const uint32_t d = s.cand[idx];
-                            XgmBlockHdr bh;
-                            uint32_t nf;
-                            const uint32_t b = warp_seek(lh, lo, lnblk, d, lane, bh, nf);
-                            if (d < bh.first) continue;
-                            const uint32_t dbits = XGM_HDR_DOC_BITS(bh.meta), cnt = XGM_HDR_COUNT(bh.meta);
-                            stage_issue(0, p.docs, bh.doc_off, dbits);
-                            stage_wait(0, dbits);
-                            uint32_t bd[4];
-                            decode_docids(s.stage[warp][0], dbits, bh.first, lane, bd);
-                            uint32_t found = 0;
-#pragma unroll
-                            for (int k = 0; k < 4; ++k)
-                                if (4 * lane + k < cnt && bd[k] == d) found = 4 * lane + k + 1;
-                            const uint32_t bal = __ballot_sync(FULL, found != 0);
-                            if (bal) {
-                                const uint32_t pos = __shfl_sync(FULL, found, __ffs(bal) - 1) - 1;
-                                if (lane == 0) {
-                                    s.hitpos[idx] = ((b - lo) << 7) | pos;
-                                    atomicOr(&s.hit[idx >> 5], 1u << (idx & 31));
-                                }
-                            }
-                            __syncwarp();
-                        }
-                    }
-                }
-            }
-            __syncthreads();
-            /* resolve: survivors = alive & hit; score them (MultiAndPostList::get_weight order) */
-            for (uint32_t idx = tid; idx < nb * XGM_BLOCK; idx += A2_THREADS) {
-                const uint32_t m = 1u << (idx & 31);
-                if ((s.alive[idx >> 5] & m) && (s.hit[idx >> 5] & m)) {
-                    const uint32_t d = s.cand[idx];
-                    const uint32_t dlen = __ldg(&p.doclen[d]);
-                    if (j == 1) {
-                        const XgmBlockHdr dh = hdr[drv_begin + wi.b0 + (idx >> 7)];
-                        const uint32_t tf0 = unpack_gl(p.tfs, dh.tf_off, idx & 127u, XGM_HDR_TF_BITS(dh.meta));
-                        s.acc[idx] = bm25_sumpart(tw0, q, tf0, dlen);
-                    }
-                    uint32_t bj, pj; /* block and position of the posting in list j */
-                    if (has_bm) {
-                        /* rank of docid d = postings before its 256-docid group + set bits before it */
-                        const uint32_t* __restrict__ bm = p.bitmaps + q->terms[j].bm_off;
-                        const uint32_t g = d >> 8, wsel = (d >> 5) & 7u;
-                        uint32_t r = __ldg(p.ranks + q->terms[j].rk_off + g);
-                        const uint4 a = __ldg(reinterpret_cast<const uint4*>(bm + g * 8));
-                        const uint4 b2 = __ldg(reinterpret_cast<const uint4*>(bm + g * 8 + 4));
-                        const uint32_t ww[8] = {a.x, a.y, a.z, a.w, b2.x, b2.y, b2.z, b2.w};
-#pragma unroll
-                        for (uint32_t x = 0; x < 8; ++x) {
-                            if (x < wsel) r += __popc(ww[x]);
-                            else if (x == wsel) r += __popc(ww[x] & ((1u << (d & 31)) - 1u));
-                        }
-                        bj = r >> 7; pj = r & 127u;
-                    } else {
-                        const uint32_t hp = s.hitpos[idx];
-                        bj = lo + (hp >> 7); pj = hp & 127u;
-                    }
-                    const XgmBlockHdr bh = lh[bj];
-                    const uint32_t tfj = unpack_gl(p.tfs, bh.tf_off, pj, XGM_HDR_TF_BITS(bh.meta));
-                    s.acc[idx] = __dadd_rn(s.acc[idx], bm25_sumpart(twj, q, tfj, dlen));
-                }
-            }
-            __syncthreads();
-            if (tid < A2_CAND / 32) { s.alive[tid] &= s.hit[tid]; s.hit[tid] = 0u; }
-            __syncthreads();
-        }
-
-        /* ---- filter + emit: warp w handles driver blocks w, w+8 ---- */
-        for (uint32_t blk = warp; blk < nb; blk += A2_WARPS) {
-            uint32_t alive = 0, c[4];
-            double acc[4];
-            const uint32_t aw = s.alive[blk * 4 + (lane >> 3)];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const uint32_t idx = blk * XGM_BLOCK + 4 * lane + k;
-                c[k] = s.cand[idx];
-                acc[k] = s.acc[idx];
-                if (aw >> ((4 * lane + k) & 31) & 1u) alive |= 1u << k;
-            }
-            if (q->filter) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    if ((alive >> k & 1u) && !doc_passes_filter(p, q, c[k])) alive &= ~(1u << k);
-            }
-            const uint32_t aux[4] = {nterms, nterms, nterms, nterms};
-            emit_matches(p, q, wi.query, lane, alive, acc, c, aux);
-        }
-    }
-}
-
-cudaError_t xgm_launch_and2(const XgmKernelParams& p, int grid, cudaStream_t s) {
-    cudaError_t e = optin_smem((const void*)xgm_and2_kernel, 2, sizeof(A2Smem));
-    if (e != cudaSuccess) return e;
-    xgm_and2_kernel<<<grid, A2_THREADS, sizeof(A2Smem), s>>>(p);
-    return cudaGetLastError();
-}
-
-int xgm_and2_occupancy_blocks_per_sm() {
-    int n = 0;
-    cudaFuncSetAttribute(xgm_and2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(A2Smem));
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_and2_kernel, A2_THREADS, sizeof(A2Smem));
+    cudaFuncSetAttribute(xgm_and_bm3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_and_bm3_kernel, BM3_WARPS * 32, smem);
     return n;
 }
 
