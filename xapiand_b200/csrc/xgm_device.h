@@ -17,11 +17,30 @@ struct XgmDevResult {
     uint32_t n;      /* entries written to out_* (<= topk) */
     uint32_t exact;  /* documents matching the boolean structure */
     uint32_t known;  /* ProtoMSet::known_matching_docs */
-    uint32_t flags;  /* bit0: candidates were lost (buffer overflow); bit1: match-count bounds approximate */
+    uint32_t flags;  /* XGM_RES_* */
     double max_w;    /* dense kernel: best weight seen */
     uint32_t max_subqs;
     uint32_t pad;
 };
+#define XGM_RES_LOST 1u        /* candidates were lost: the overflow pool could not take the second pass */
+#define XGM_RES_APPROX 2u      /* the match-count bounds are approximate (pruned run) */
+#define XGM_RES_PENDING 4u     /* the first pass overflowed: a second pass is pending */
+#define XGM_RES_SKIPPED 8u     /* whole work items were skipped by MaxScore: the match count is a lower bound */
+#define XGM_RES_SECOND_PASS 16u /* produced by the second pass */
+
+/* Slots of XgmKernelParams::work_counter, zeroed before every batch.  A counter of per-pass work has one slot per
+ * pass, slot + pass. */
+#define XGM_WC_AND 0        /* [0],[1]   items of xgm_and_kernel taken */
+#define XGM_WC_OR 2         /* [2],[3]   items of xgm_or_kernel taken */
+#define XGM_WC_RERUN 4      /* [4]       queries the second pass re-runs */
+#define XGM_WC_AND_BM 6     /* [6],[7]   items of xgm_and_bm3_kernel taken */
+#define XGM_WC_POOL 8       /* [8..9]    64-bit overflow-pool reservation, in entries */
+#define XGM_WC_OR3 10       /* [10],[11] items of xgm_or3_kernel<0> taken */
+#define XGM_WC_TILE 12      /* [12],[13] tiles of xgm_or_tile_kernel taken */
+#define XGM_WC_OR3_SINGLE 14 /* [14],[15] items of xgm_or3_kernel<1> taken */
+#define XGM_WC_TOPK_FRONT 16 /* [16]      topk_list entries written from the front */
+#define XGM_WC_TOPK 17      /* [17],[18] entries handed to the CTAs of xgm_topk_kernel */
+#define XGM_WC_TOPK_BACK 19 /* [19]      topk_list entries written from the back */
 
 struct XgmKernelParams {
     /* index */
@@ -46,7 +65,7 @@ struct XgmKernelParams {
      * its one query. */
     const XgmWorkItem* bm_segs;
     uint32_t nq;
-    uint32_t* work_counter;       /* [10],[11] OR items of xgm_or3_kernel (first / second pass); [12],[13] tiles of xgm_or_tile_kernel; [14],[15] items of xgm_or3_kernel<PHASE 1>; [8..9] 64-bit pool reservation; [0] AND items, [1] OR items, [2],[3] same for the second pass, [4] #queries to re-run, [5] overflow-pool entries reserved, [6],[7] bitmap-AND items (first / second pass) */
+    uint32_t* work_counter;       /* batch counters, slots XGM_WC_* */
     uint32_t pass;                /* 0 = first pass, 1 = re-run of overflowed queries with their exact b* */
     XgmQState* qstate;            /* [nq] */
     uint32_t* hist;               /* [nq][XGM_NBINS] */
@@ -68,20 +87,23 @@ struct XgmKernelParams {
     uint64_t* out_k;
     XgmDevResult* out_info;
     XgmRaise* raise_log;          /* [nq][XGM_RAISE_LOG] */
-    const uint32_t* tileq;        /* queries answered by xgm_or_tile_kernel + xgm_or3_kernel<PHASE 1> */
+    /* xgm_or_tile_kernel's work list: the queries with or_fast == XGM_OR_FAST_TILE (xgm_or3_kernel<1> finds their
+     * items in items_or) */
+    const uint32_t* tileq;
     uint32_t ntileq;
-    /* top-k: queries xgm_topk_small_kernel left to xgm_topk_kernel (work_counter[16] expensive ones from the front
-     * of the list, [19] others from its back); null = every query of the batch.  work_counter[17 + pass] hands the
-     * entries out. */
+    /* top-k: queries xgm_topk_small_kernel left to xgm_topk_kernel (XGM_WC_TOPK_FRONT counts the expensive ones from
+     * the front of the list, XGM_WC_TOPK_BACK the others from its back); null = every query of the batch.
+     * XGM_WC_TOPK + pass hands the entries out. */
     uint32_t* topk_list;
 };
 #define XGM_CTRL_HDR 128 /* bytes of work counters in front of the per-query state */
+static_assert(4 * (XGM_WC_TOPK_BACK + 1) <= XGM_CTRL_HDR, "the work counters fit their header");
 
 cudaError_t xgm_launch_and(const XgmKernelParams& p, int grid, cudaStream_t s);
 cudaError_t xgm_launch_and_bm(const XgmKernelParams& p, int grid, cudaStream_t s);
 int xgm_and_bm_occupancy_blocks_per_sm();
-cudaError_t xgm_launch_expand(const XgmWorkItem* seg, uint32_t nseg, uint32_t total, const uint32_t* level_start,
-                              uint32_t nlevels, uint32_t bpi, XgmWorkItem* out, cudaStream_t s);
+cudaError_t xgm_launch_expand(const XgmWorkItem* seg, uint32_t total, const uint32_t* level_start, uint32_t nlevels,
+                              uint32_t bpi, XgmWorkItem* out, cudaStream_t s);
 cudaError_t xgm_launch_expand_ranges(const XgmWorkItem* runs, uint32_t nruns, const XgmBlockHdr* hdr, uint32_t nranges,
                                      uint32_t range_bits, uint32_t bpi, uint32_t* lo, uint32_t* cnt, uint32_t* off,
                                      uint32_t* total, XgmWorkItem* out, cudaStream_t s);

@@ -52,6 +52,16 @@ struct XgmDevTerm {
     double maxpart;       /* BM25Weight::get_maxpart: upper bound of the term's contribution (MaxScore pruning) */
 };
 
+/* XgmDevQuery::route: the shape of the query on the device */
+#define XGM_ROUTE_AND 0u /* required lists (then excluded and optional ones): the AND kernels */
+#define XGM_ROUTE_OR 1u  /* OrPostList tree over the leaves: the OR kernels */
+
+/* XgmDevQuery::or_fast: which kernels produce an OR's union */
+#define XGM_OR_FAST_GENERAL 0u /* xgm_or_kernel: a leaf without bitmap, more than five leaves, or filter / AND_NOT terms */
+#define XGM_OR_FAST_OR3 1u     /* xgm_or3_kernel<0>: at most five leaves, all with bitmaps */
+#define XGM_OR_FAST_TILE 2u    /* as OR3 in relevance order with results and no value range: xgm_or_tile_kernel for
+                                  the documents with two or more leaves, then xgm_or3_kernel<1> for the rest */
+
 struct XgmDevQuery {
     uint32_t op, nterms, topk, check_at_least;
     double len_factor, k1, b, one_minus_b, min_normlen;
@@ -60,7 +70,7 @@ struct XgmDevQuery {
     uint32_t sort_by, sort_slot, sort_reverse, sort_use_max;
     uint32_t prog_len;
     int8_t prog[2 * XGM_DEV_MAX_TERMS]; /* OR: postfix program over leaves (>=0) and '+' (-1) */
-    uint32_t route;                     /* 0 = AND kernel, 1 = OR kernel */
+    uint32_t route;                     /* XGM_ROUTE_AND or XGM_ROUTE_OR */
     uint32_t nnot;                      /* AND: terms[nterms .. nterms+nnot) must be absent (OP_AND_NOT right side) */
     uint32_t nweighted;                 /* required leaves that carry a weight (OP_FILTER's boolean terms do not) */
     uint32_t nmaybe;                    /* AND: terms[nterms+nnot ..) are the optional leaves of an OP_AND_MAYBE; prog[] is
@@ -71,7 +81,7 @@ struct XgmDevQuery {
     double src_weight;                  /* weighted value-range source: factor * 1.0 added to every match ... */
     uint32_t src_pos;                   /* ... before the weight of required list src_pos (MultiAndPostList order);
                                            nterms = after all; XGM_NO_SRC = the source only filters */
-    uint32_t or_fast;                   /* OR: every leaf has a membership bitmap and there are at most 5 → xgm_or3_kernel */
+    uint32_t or_fast;                   /* OR: the kernels that produce its union, XGM_OR_FAST_* */
     uint32_t or_nreq;                   /* OR under OP_FILTER: terms[nterms .. nterms+or_nreq) must hold the document, then nnot excluded ones */
     uint32_t log_raises;                /* record the matches that attain the running maximum weight (XGM_RAISE_LOG) */
     XgmDevTerm terms[XGM_DEV_MAX_TERMS]; /* AND: ascending termfreq (MultiAndPostList order) */

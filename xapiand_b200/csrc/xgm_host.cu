@@ -974,7 +974,7 @@ struct WorkList {
 
 /* The OR list: one level-ordered expansion per leaf position */
 struct OrList : WorkList {
-    struct Group { uint32_t seg_off, nseg, level_off, nlevels, out_off, total; };
+    struct Group { uint32_t seg_off, level_off, nlevels, out_off, total; };
     std::vector<Group> groups;
 };
 
@@ -1495,7 +1495,7 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
         pq.tf_est = ix->doccount ? (uint32_t)(r + 0.5) : 0;
         if (src_weighted) { dq.src_pos = src_pos; dq.src_weight = src_w; }
         pq.mv_source = mv_source;
-        dq.route = 0;
+        dq.route = XGM_ROUTE_AND;
         auto put_term = [&](uint32_t slot, uint32_t j, bool weighted) {
             dq.terms[slot].termweight = weighted ? tw[j] : 0.0; /* a boolean leaf contributes +0.0: sums unchanged */
             dq.terms[slot].maxpart = weighted ? maxpart[j] : 0.0;
@@ -1620,7 +1620,7 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
         }
         pq.max_possible = sm[0]; pq.tf_min = smin[0]; pq.tf_max = smax[0]; pq.tf_est = (uint32_t)se[0];
         pq.bucket_max = pq.max_possible;
-        dq.route = 1;
+        dq.route = XGM_ROUTE_OR;
         auto put_leaf = [&](uint32_t slot, uint32_t j, bool weighted) {
             dq.terms[slot].termweight = weighted ? tw[j] : 0.0;
             dq.terms[slot].maxpart = weighted ? maxpart[j] : 0.0;
@@ -1674,14 +1674,14 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
 
     /* percent_scale_factor needs the number of subqueries matching the best-WEIGHTED document: when that varies
      * per document and the order is not by weight alone, have the kernels log the running-maximum matches */
-    dq.log_raises = ((dq.route == 1 && n > 1) || pq.aux_subqs) && q.sort_by != XGM_SORT_REL ? 1u : 0u;
+    dq.log_raises = ((dq.route == XGM_ROUTE_OR && n > 1) || pq.aux_subqs) && q.sort_by != XGM_SORT_REL ? 1u : 0u;
     pq.log_raises = dq.log_raises != 0;
     if (cal == 0) { pq.on_device = false; return XGM_OK; } /* bounds only, matcher.cc:437-461 */
-    if (dq.route == 0 && any_absent) { pq.on_device = false; return XGM_OK; } /* AND with an absent term: empty */
-    if (dq.route == 1 && group_absent) { pq.on_device = false; return XGM_OK; } /* OR filtered by an absent term: empty */
+    if (dq.route == XGM_ROUTE_AND && any_absent) { pq.on_device = false; return XGM_OK; } /* AND with an absent term: empty */
+    if (dq.route == XGM_ROUTE_OR && group_absent) { pq.on_device = false; return XGM_OK; } /* OR filtered by an absent term: empty */
     pq.on_device = true;
     /* one segment per (query[, leaf]); the device expands segments into work items (xgm_expand_items_kernel) */
-    if (dq.route == 0) {
+    if (dq.route == XGM_ROUTE_AND) {
         /* every list but the driver has a membership bitmap → lean bitmap kernel */
         bool all_bm = dq.nterms >= 2;
         for (uint32_t i = 1; i < dq.nterms + dq.nnot; ++i) all_bm = all_bm && dq.terms[i].bm_off != XGM_NO_BITMAP;
@@ -1692,8 +1692,9 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
     } else {
         bool fastor = n <= 5 && ngroups == 0 && !(getenv("XGM_OR_KERNEL") && atoi(getenv("XGM_OR_KERNEL")) == 1);
         for (uint32_t leaf = 0; leaf < n; ++leaf) fastor = fastor && dq.terms[leaf].bm_off != XGM_NO_BITMAP;
-        /* relevance order, no predicate, results wanted: multi-leaf documents by bitmap union first (or_fast 2) */
-        dq.or_fast = !fastor ? 0u : (s->or_tile && q.filter == XGM_FILTER_NONE && q.sort_by == XGM_SORT_REL && dq.topk != 0) ? 2u : 1u;
+        /* relevance order, no predicate, results wanted: multi-leaf documents by bitmap union first */
+        const bool tile = s->or_tile && q.filter == XGM_FILTER_NONE && q.sort_by == XGM_SORT_REL && dq.topk != 0;
+        dq.or_fast = !fastor ? XGM_OR_FAST_GENERAL : tile ? XGM_OR_FAST_TILE : XGM_OR_FAST_OR3;
         for (uint32_t leaf = 0; leaf < n; ++leaf) {
             XgmWorkItem wi;
             wi.query = qi; wi.b0 = dq.terms[leaf].nblocks; wi.b1 = 0; wi.pad = leaf;
@@ -1760,7 +1761,7 @@ static xgm_status order_or_groups(OrList& L, std::vector<XgmWorkItem>& v, uint32
         size_t b = a;
         while (b < v.size() && v[b].pad == v[a].pad) ++b;
         OrList::Group g;
-        g.seg_off = (uint32_t)a; g.nseg = (uint32_t)(b - a); g.level_off = (uint32_t)lvpos;
+        g.seg_off = (uint32_t)a; g.level_off = (uint32_t)lvpos;
         g.nlevels = (v[a].b0 + bpi - 1) / bpi;
         g.out_off = (uint32_t)run;
         const uint64_t n = level_starts(v.data() + a, b - a, g.nlevels, bpi, L.levels.h + lvpos);
@@ -1827,12 +1828,12 @@ static xgm_status order_driver_runs(xgm_searcher* s, std::vector<XgmWorkItem>& v
 static cudaError_t expand_levels(const WorkList& L, uint32_t bpi, cudaStream_t cs, uint32_t& launches) {
     if (!L.nitems) return cudaSuccess;
     ++launches;
-    return xgm_launch_expand(L.seg.d, L.nseg, L.nitems, L.levels.d, L.nstarts - 1, bpi, L.d_exp, cs);
+    return xgm_launch_expand(L.seg.d, L.nitems, L.levels.d, L.nstarts - 1, bpi, L.d_exp, cs);
 }
 
 static cudaError_t expand_or_groups(const OrList& L, uint32_t bpi, cudaStream_t cs, uint32_t& launches) {
     for (const auto& g : L.groups) {
-        cudaError_t e = xgm_launch_expand(L.seg.d + g.seg_off, g.nseg, g.total, L.levels.d + g.level_off, g.nlevels, bpi,
+        cudaError_t e = xgm_launch_expand(L.seg.d + g.seg_off, g.total, L.levels.d + g.level_off, g.nlevels, bpi,
                                           L.d_exp + g.out_off, cs);
         if (e != cudaSuccess) return e;
         ++launches;
@@ -1947,7 +1948,7 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     }
     const auto t_planned = std::chrono::steady_clock::now();
     for (uint32_t i = 0; i < nq; ++i) {
-        if (s->plan[i].sort_by || s->h_queries[i].route == 1 || s->plan[i].aux_subqs) s->any_sort = true; /* keys/aux needed on the host */
+        if (s->plan[i].sort_by || s->h_queries[i].route == XGM_ROUTE_OR || s->plan[i].aux_subqs) s->any_sort = true; /* keys/aux needed on the host */
         alg += s->plan[i].alg_bytes;
     }
     /* segments → each list's pinned staging, in the order the device expands them */
@@ -1986,9 +1987,9 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     s->any_or_fast = s->any_or_slow = false;
     s->ntileq = 0;
     for (uint32_t i = 0; i < nq; ++i)
-        if (s->h_queries[i].route == 1 && s->plan[i].on_device) {
-            if (s->h_queries[i].or_fast == 2) s->h_tileq[s->ntileq++] = i;
-            else if (s->h_queries[i].or_fast) s->any_or_fast = true;
+        if (s->h_queries[i].route == XGM_ROUTE_OR && s->plan[i].on_device) {
+            if (s->h_queries[i].or_fast == XGM_OR_FAST_TILE) s->h_tileq[s->ntileq++] = i;
+            else if (s->h_queries[i].or_fast == XGM_OR_FAST_OR3) s->any_or_fast = true;
             else s->any_or_slow = true;
         }
     p.tileq = s->d_tileq; p.ntileq = s->ntileq;
@@ -2054,9 +2055,9 @@ static void finish_info(const PlannedQuery& pq, const XgmDevResult* dr, const do
          * more: our count is then a lower bound — flag the bounds. */
         if (pq.check_at_least > pq.topk + 1 && known < dr->exact && !pq.count_only && pq.sort_by == XGM_SORT_REL_VAL)
             o->flags |= XGM_MSET_BOUNDS_APPROX; /* relevance-then-value still uses the simple counting rule */
-        if (dr->flags & 5u) o->status = XGM_E_UNIMPLEMENTED; /* candidates lost: pathological tie mass */
-        if (dr->flags & 2u) o->flags |= XGM_MSET_BOUNDS_APPROX;
-        if (dr->flags & 8u) o->flags |= XGM_MSET_BOUNDS_APPROX | XGM_MSET_COUNT_LOWER_BOUND;
+        if (dr->flags & (XGM_RES_LOST | XGM_RES_PENDING)) o->status = XGM_E_UNIMPLEMENTED; /* lost or pending: pathological tie mass */
+        if (dr->flags & XGM_RES_APPROX) o->flags |= XGM_MSET_BOUNDS_APPROX;
+        if (dr->flags & XGM_RES_SKIPPED) o->flags |= XGM_MSET_BOUNDS_APPROX | XGM_MSET_COUNT_LOWER_BOUND;
         /* with a value-range source in the AND the reference's lower bound / estimate also fold in
          * ValueRangePostList::get_termfreq_est (valuerangepostlist.cc:70-130), which is not restated */
         if (pq.filter && !pq.mv_source && size == pq.topk && known >= pq.check_at_least) o->flags |= XGM_MSET_BOUNDS_APPROX;
@@ -2195,9 +2196,9 @@ extern "C" xgm_status xgm_search_wait(xgm_searcher* s, uint32_t* docids, double*
     for (uint32_t i = 0; i < s->nq; ++i) {
         const PlannedQuery& pq = s->plan[i];
         const size_t off = (size_t)i * s->max_topk;
-        if (pq.status == XGM_OK && pq.on_device && (s->h_info[i].flags & 16u)) s->stats.second_pass_queries++;
+        if (pq.status == XGM_OK && pq.on_device && (s->h_info[i].flags & XGM_RES_SECOND_PASS)) s->stats.second_pass_queries++;
         finish_info(pq, &s->h_info[i], s->h_out_w + off, s->any_sort ? s->h_out_k + off : nullptr,
-                    s->h_queries[i].route == 1 || pq.aux_subqs, &info[i],
+                    s->h_queries[i].route == XGM_ROUTE_OR || pq.aux_subqs, &info[i],
                     s->any_raise ? s->h_raise + (size_t)i * XGM_RAISE_LOG : nullptr, s->any_raise ? s->h_qstate[i].nraise : 0u);
         if (pq.status == XGM_OK && pq.on_device) s->stats.algorithmic_bytes += 4ull * s->h_info[i].exact;
         uint32_t n = info[i].n;

@@ -1,12 +1,19 @@
 /* xgm_kernels.cu — sm_90a (H100) kernels of the matcher hot path.
  *
- *   xgm_and_kernel    decode + warp-galloping intersection + fused BM25 (reference:
- *                     GlassPostList::next/skip_to glass_postlist.cc:768-991, MultiAndPostList::
- *                     find_next_match multiandpostlist.cc:179-206, get_weight :149-159,
- *                     BM25Weight::get_sumpart bm25weight.cc:170-181, doclen fetch postlisttree.h:184-195)
- *   xgm_or_kernel     owner-leaf union with the reference's tree-order sum (OrPostList, orpostlist.cc:93-204)
- *   xgm_topk_kernel   ProtoMSet top-k + match counting (protomset.h:295-400,484-683; msetcmp.cc:54-98)
- *   xgm_decode_kernel round-trip decode of one term (index self-check)
+ *   xgm_and_kernel          decode + warp-galloping intersection + fused BM25 (reference:
+ *                           GlassPostList::next/skip_to glass_postlist.cc:768-991, MultiAndPostList::
+ *                           find_next_match multiandpostlist.cc:179-206, get_weight :149-159,
+ *                           BM25Weight::get_sumpart bm25weight.cc:170-181, doclen fetch postlisttree.h:184-195)
+ *   xgm_and_bm3_kernel      the same AND when every list but the driver has a membership bitmap
+ *   xgm_or_kernel           owner-leaf union with the reference's tree-order sum (OrPostList, orpostlist.cc:93-204)
+ *   xgm_or3_kernel          the same OR for at most five leaves, all with bitmaps
+ *   xgm_or_tile_kernel      documents with two or more leaves of such an OR, by bitmap union
+ *   xgm_topk_small_kernel   ProtoMSet top-k + match counting (protomset.h:295-400,484-683; msetcmp.cc:54-98):
+ *   xgm_topk_kernel         a warp per query with a handful of matches, a CTA per query otherwise
+ *   xgm_merge_kernel        merge of the per-shard top-k lists (Matcher::merge_mset)
+ *   xgm_decode_kernel       round-trip decode of one term (index self-check)
+ *   xgm_expand_items_kernel work items of a level-ordered list from its segments
+ *   xgm_range_{count,scan,fill}_kernel   work items of the range-major bitmap AND list
  *
  * Integer/pointer work: no tensor cores. Packed blocks are staged global→shared with the bulk-copy
  * engine (cp.async.bulk + mbarrier, SASS UBLKCP), deltas are undone with a warp prefix sum, every
@@ -43,31 +50,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "XGM_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-        "@P1 bra XGM_DONE;\n"
-        "bra XGM_WAIT;\n"
-        "XGM_DONE:\n"
-        "}" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-
-/* the same on precomputed shared-space addresses (hot loops: no generic→shared conversion per call) */
+/* on shared-space addresses (hot loops precompute them: no generic→shared conversion per call) */
 __device__ __forceinline__ void mbar_expect_tx_a(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -89,6 +72,11 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
         "r"(parity)
         : "memory");
 }
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) { mbar_expect_tx_a(smem_u32(bar), bytes); }
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    bulk_g2s_a(smem_u32(dst), src, bytes, smem_u32(bar));
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { mbar_wait_a(smem_u32(bar), parity); }
 
 /* ------------------------------------------------------------------ block decode */
 
@@ -404,15 +392,11 @@ __device__ __forceinline__ void emit_matches(const XgmKernelParams& p, const Xgm
 
 #define MATCH_WARPS 8
 
+/* what stage_block and probe_list use */
 struct __align__(16) WarpScratch {
     uint32_t stage[STAGE_WORDS];      /* packed words of the block being probed */
-    uint32_t dstage[2][STAGE_WORDS];  /* double-buffered packed docids of the driver list */
     uint32_t dbuf[XGM_BLOCK];         /* decoded docids of the probed block */
-    uint32_t qdid[160];               /* bitmap fast path: queue of candidates confirmed by the second list */
-    uint32_t qsrc[160];               /*   (driver block - b0) << 7 | position, for the lazy wdf fetch */
     uint64_t bar;                     /* completion barrier of `stage` */
-    uint64_t dbar[2];                 /* completion barriers of `dstage` */
-    uint64_t pad;
 };
 
 __device__ __forceinline__ void issue_stage(const uint4* col, uint32_t off16, uint32_t bits, uint32_t* st, uint64_t* bar,
@@ -530,27 +514,20 @@ __device__ __noinline__ bool lookup_posting(const XgmKernelParams& p, const XgmD
     return true;
 }
 
-/* AndMaybePostList::get_weight (matcher/andmaybepostlist.cc:59-67): the right side's weight, i.e. the
- * OrPostList tree (l, r or l + r per node, matcher/orpostlist.cc:93-103) over the optional leaves that hold
- * docid d, evaluated as the postfix program built on the host.  *present = how many leaves matched. */
-__device__ __noinline__ double maybe_weight(const XgmKernelParams& p, const XgmDevQuery* q, uint32_t d, uint32_t dlen,
-                                            uint32_t* present) {
+/* OrPostList::get_weight (matcher/orpostlist.cc:93-103): the tree over the leaves that hold the document, l, r or
+ * l + r per node, evaluated as the postfix program q->prog built on the host (leaf >= 0, '+' = -1).  leaf(op, v)
+ * returns whether leaf op holds the document and, if it does, sets v to the leaf's weight.  The result is only
+ * defined when some leaf holds the document: the callers know whether one does. */
+template <class Leaf>
+__device__ __forceinline__ double or_tree_weight(const XgmDevQuery* q, Leaf leaf) {
     double stk[XGM_DEV_MAX_TERMS];
-    uint32_t has = 0, cnt = 0;
+    uint32_t has = 0; /* bit s: stack slot s holds a value */
     int sp = 0;
-    const uint32_t base = q->nterms + q->nnot;
     for (uint32_t i = 0; i < q->prog_len; ++i) {
         const int op = q->prog[i];
         if (op >= 0) {
-            const XgmDevTerm& t = q->terms[base + (uint32_t)op];
-            uint32_t wdf = 0;
-            if (lookup_posting(p, t, d, &wdf)) {
-                stk[sp] = bm25_sumpart(t.termweight, q, wdf, dlen);
-                has |= 1u << sp;
-                ++cnt;
-            } else {
-                has &= ~(1u << sp);
-            }
+            if (leaf((uint32_t)op, stk[sp])) has |= 1u << sp;
+            else has &= ~(1u << sp);
             ++sp;
         } else {
             --sp;
@@ -559,26 +536,54 @@ __device__ __noinline__ double maybe_weight(const XgmKernelParams& p, const XgmD
             else if (hr) { stk[sp - 1] = stk[sp]; has |= 1u << (sp - 1); }
         }
     }
+    return stk[0];
+}
+
+/* AndMaybePostList::get_weight (matcher/andmaybepostlist.cc:59-67): the right side's weight, i.e. the
+ * OrPostList tree over the optional leaves that hold docid d.  *present = how many leaves matched. */
+__device__ __noinline__ double maybe_weight(const XgmKernelParams& p, const XgmDevQuery* q, uint32_t d, uint32_t dlen,
+                                            uint32_t* present) {
+    /* wdf is declared here, not in the lambda, so that it follows the fold's stack in the frame: with the other
+     * order ptxas gives xgm_and_bm3_kernel, which calls this function, a 176-byte frame and spills instead of 160 */
+    uint32_t cnt = 0, wdf;
+    const uint32_t base = q->nterms + q->nnot;
+    const double w = or_tree_weight(q, [&](uint32_t op, double& v) {
+        const XgmDevTerm& t = q->terms[base + op];
+        wdf = 0;
+        if (!lookup_posting(p, t, d, &wdf)) return false;
+        v = bm25_sumpart(t.termweight, q, wdf, dlen);
+        ++cnt;
+        return true;
+    });
     *present = cnt;
-    return cnt ? stk[0] : 0.0;
+    return cnt ? w : 0.0;
 }
 
 /* ------------------------------------------------------------------ sparse AND kernel */
 
+struct __align__(16) AndScratch {
+    WarpScratch w;
+    uint32_t dstage[2][STAGE_WORDS];  /* double-buffered packed docids of the driver list */
+    uint64_t dbar[2];                 /* completion barriers of `dstage` */
+};
+
+/* The planner sends every AND whose lists but the driver all have bitmaps to xgm_and_bm3_kernel: here some list
+ * has none, or the query has a single term. */
 __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(XgmKernelParams p) {
-    __shared__ WarpScratch scratch[MATCH_WARPS];
+    __shared__ AndScratch scratch[MATCH_WARPS];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    WarpScratch& ws = scratch[warp];
-    if (lane == 0) { mbar_init(&ws.bar, 1); mbar_init(&ws.dbar[0], 1); mbar_init(&ws.dbar[1], 1); }
+    AndScratch& as = scratch[warp];
+    WarpScratch& ws = as.w;
+    if (lane == 0) { mbar_init(&ws.bar, 1); mbar_init(&as.dbar[0], 1); mbar_init(&as.dbar[1], 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
     uint32_t phase = 0, dphase0 = 0, dphase1 = 0;
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
 
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + 4) == 0) return; /* nothing to re-run */
+    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return; /* nothing to re-run */
     for (;;) {
         uint32_t item = 0;
-        if (lane == 0) item = atomicAdd(p.work_counter + 2 * p.pass, 1u);
+        if (lane == 0) item = atomicAdd(p.work_counter + XGM_WC_AND + p.pass, 1u);
         item = __shfl_sync(FULL, item, 0);
         if (item >= p.nitems) break;
         const XgmWorkItem wi = p.items[item];
@@ -594,114 +599,30 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(XgmKernelP
         const uint32_t drv_begin = __shfl_sync(FULL, my_begin, 0);
         const double tw0 = q->terms[0].termweight;
 
-        /* Fast path when every other list has a membership bitmap: the intersection is a word load per
-         * candidate; candidates confirmed by the second list are queued and finished 32 at a time (one
-         * per lane) so that the rank / wdf / BM25 work of the few survivors runs on full warps. */
-        bool fast = nterms >= 2;
-        for (uint32_t j = 1; j < nterms + nnot; ++j) fast = fast && (q->terms[j].bm_off != XGM_NO_BITMAP);
-        uint32_t qn = 0;
-        auto flush = [&](uint32_t from, uint32_t count) {
-            uint32_t alive = lane < count ? 1u : 0u;
-            const uint32_t d = alive ? ws.qdid[from + lane] : 0u;
-            const uint32_t src = alive ? ws.qsrc[from + lane] : 0u;
-            for (uint32_t j = 2; j < nterms + nnot && __any_sync(FULL, alive); ++j) {
-                if (alive) {
-                    const uint32_t w = __ldg(p.bitmaps + q->terms[j].bm_off + (d >> 5));
-                    /* required lists must hold the docid; the right side of an OP_AND_NOT must not
-                     * (AndNotPostList::next, matcher/andnotpostlist.cc:97-130) */
-                    if (((w >> (d & 31)) & 1u) == (j < nterms ? 0u : 1u)) alive = 0u;
-                }
-            }
-            if (alive && q->filter && !doc_passes_filter(p, q, d)) alive = 0u;
-            double acc[4] = {0.0, 0.0, 0.0, 0.0};
-            uint32_t opt = 0;
-            if (alive) {
-                const uint32_t dlen = __ldg(&p.doclen[d]);
-                const XgmBlockHdr h0 = hdr[drv_begin + wi.b0 + (src >> 7)];
-                const uint32_t sp = q->src_pos; /* weighted range source: the child at this place of the sum */
-                if (sp == 0) acc[0] = q->src_weight;
-                acc[0] = __dadd_rn(acc[0], bm25_sumpart(tw0, q, unpack_gl(p.tfs, h0.tf_off, src & 127u, XGM_HDR_TF_BITS(h0.meta)), dlen));
-                for (uint32_t j = 1; j < nterms; ++j) {
-                    if (sp == j) acc[0] = __dadd_rn(acc[0], q->src_weight);
-                    const uint32_t r = bitmap_rank(p, q->terms[j], d);
-                    const XgmBlockHdr bh = hdr[q->terms[j].blk_begin + (r >> 7)];
-                    const uint32_t tfj = unpack_gl(p.tfs, bh.tf_off, r & 127u, XGM_HDR_TF_BITS(bh.meta));
-                    /* MultiAndPostList::get_weight: result += plist[i]->get_weight(), in plist order */
-                    acc[0] = __dadd_rn(acc[0], bm25_sumpart(q->terms[j].termweight, q, tfj, dlen));
-                }
-                if (sp == nterms) acc[0] = __dadd_rn(acc[0], q->src_weight);
-                if (q->nmaybe) { /* OP_AND_MAYBE: res = l; if (r matches) res += r */
-                    const double rw = maybe_weight(p, q, d, dlen, &opt);
-                    if (opt) acc[0] = __dadd_rn(acc[0], rw);
-                }
-            }
-            const uint32_t cc[4] = {d, 0u, 0u, 0u};
-            const uint32_t aux[4] = {nweighted + opt, nweighted, nweighted, nweighted};
-            emit_matches(p, q, wi.query, lane, alive, acc, cc, aux);
-        };
-
         /* software pipeline over the driver list: block db+1 is in flight while db is intersected */
         XgmBlockHdr dh = hdr[drv_begin + wi.b0];
         __syncwarp();
-        issue_stage(p.docs, dh.doc_off, XGM_HDR_DOC_BITS(dh.meta), ws.dstage[0], &ws.dbar[0], lane);
+        issue_stage(p.docs, dh.doc_off, XGM_HDR_DOC_BITS(dh.meta), as.dstage[0], &as.dbar[0], lane);
         uint32_t buf = 0;
         for (uint32_t db = wi.b0; db < wi.b1; ++db) {
             XgmBlockHdr nh = dh;
             if (db + 1 < wi.b1) {
                 nh = hdr[drv_begin + db + 1];
                 __syncwarp();
-                issue_stage(p.docs, nh.doc_off, XGM_HDR_DOC_BITS(nh.meta), ws.dstage[buf ^ 1], &ws.dbar[buf ^ 1], lane);
+                issue_stage(p.docs, nh.doc_off, XGM_HDR_DOC_BITS(nh.meta), as.dstage[buf ^ 1], &as.dbar[buf ^ 1], lane);
             }
             const uint32_t dbits = XGM_HDR_DOC_BITS(dh.meta);
             if (dbits) {
-                if (buf == 0) { mbar_wait(&ws.dbar[0], dphase0); dphase0 ^= 1u; }
-                else { mbar_wait(&ws.dbar[1], dphase1); dphase1 ^= 1u; }
+                if (buf == 0) { mbar_wait(&as.dbar[0], dphase0); dphase0 ^= 1u; }
+                else { mbar_wait(&as.dbar[1], dphase1); dphase1 ^= 1u; }
             }
             const uint32_t dcount = XGM_HDR_COUNT(dh.meta);
             uint32_t c[4];
-            decode_docids(ws.dstage[buf], dbits, dh.first, lane, c);
+            decode_docids(as.dstage[buf], dbits, dh.first, lane, c);
             uint32_t alive = 0;
 #pragma unroll
             for (int k = 0; k < 4; ++k)
                 if (4 * lane + k < dcount) alive |= 1u << k;
-
-            if (fast) {
-                const uint32_t* __restrict__ bm1 = p.bitmaps + q->terms[1].bm_off;
-                uint32_t w[4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) w[k] = (alive >> k & 1u) ? __ldg(bm1 + (c[k] >> 5)) : 0u;
-                uint32_t surv = 0;
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    if ((alive >> k & 1u) && (w[k] >> (c[k] & 31) & 1u)) surv |= 1u << k;
-                if (__any_sync(FULL, surv != 0)) {
-                    const uint32_t n = __popc(surv);
-                    uint32_t incl = n;
-#pragma unroll
-                    for (int o = 1; o < 32; o <<= 1) {
-                        const uint32_t t = __shfl_up_sync(FULL, incl, o);
-                        if ((int)lane >= o) incl += t;
-                    }
-                    uint32_t slot = qn + incl - n;
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        if (surv >> k & 1u) {
-                            ws.qdid[slot] = c[k];
-                            ws.qsrc[slot] = ((db - wi.b0) << 7) | (4 * lane + k);
-                            ++slot;
-                        }
-                    qn += __shfl_sync(FULL, incl, 31);
-                    __syncwarp();
-                    while (qn >= 32) {
-                        qn -= 32;
-                        flush(qn, 32);
-                        __syncwarp();
-                    }
-                }
-                dh = nh;
-                buf ^= 1u;
-                continue;
-            }
 
             double acc[4] = {0.0, 0.0, 0.0, 0.0};
             uint32_t dl[4] = {0, 0, 0, 0};
@@ -727,7 +648,6 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(XgmKernelP
             for (uint32_t j = 1; j < nterms; ++j) {
                 if (!__any_sync(FULL, alive != 0)) break;
                 const uint32_t lbegin = __shfl_sync(FULL, my_begin, j);
-                const uint32_t lnblk = __shfl_sync(FULL, my_nblk, j);
                 const double twj = q->terms[j].termweight;
                 auto on_hit = [&](int k, uint32_t pos, const XgmBlockHdr& bh) {
                     if (j == 1) {
@@ -755,26 +675,15 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(XgmKernelP
                     for (int k = 0; k < 4; ++k) {
                         if (alive >> k & 1u) {
                             if (w[k] >> (c[k] & 31) & 1u) {
-                                /* rank of the docid = postings before its 256-docid group + set bits before it */
-                                const uint32_t d = c[k], g = d >> 8, wsel = (d >> 5) & 7u;
-                                uint32_t r = __ldg(p.ranks + q->terms[j].rk_off + g);
-                                const uint4 a = __ldg(reinterpret_cast<const uint4*>(bm + g * 8));
-                                const uint4 b2 = __ldg(reinterpret_cast<const uint4*>(bm + g * 8 + 4));
-                                const uint32_t ww[8] = {a.x, a.y, a.z, a.w, b2.x, b2.y, b2.z, b2.w};
-#pragma unroll
-                                for (uint32_t x = 0; x < 8; ++x) {
-                                    if (x < wsel) r += __popc(ww[x]);
-                                    else if (x == wsel) r += __popc(ww[x] & ((1u << (d & 31)) - 1u));
-                                }
-                                const XgmBlockHdr bh = hdr[lbegin + (r >> 7)];
-                                on_hit(k, r & 127u, bh);
+                                const uint32_t r = bitmap_rank(p, q->terms[j], c[k]);
+                                on_hit(k, r & 127u, hdr[lbegin + (r >> 7)]);
                             } else {
                                 alive &= ~(1u << k);
                             }
                         }
                     }
-                    (void)lnblk;
                 } else {
+                    const uint32_t lnblk = __shfl_sync(FULL, my_nblk, j);
                     uint32_t cur = __shfl_sync(FULL, my_cur, j);
                     cur = probe_list(p, hdr + lbegin, lnblk, cur, ws, phase, lane, c, alive, on_hit,
                                      [&](int k) { alive &= ~(1u << k); });
@@ -821,10 +730,6 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(XgmKernelP
             emit_matches(p, q, wi.query, lane, alive, acc, c, aux);
             dh = nh;
             buf ^= 1u;
-        }
-        if (fast && qn) {
-            flush(0, qn);
-            __syncwarp();
         }
     }
 }
@@ -931,7 +836,7 @@ __device__ __forceinline__ void emit_match_lanes(const XgmKernelParams& p, uint3
                 const uint32_t after = idx + 1;
                 /* (AND: not before half of what the top-k kernel can rank is in use, so that small match sets stay
                  * unpruned and their known_matching_docs is exact; an OR's union is far larger than that anyway) */
-                crossed = (idx >> 8) != (after >> 8) && after >= q->topk && (q->route == 1 || after >= p.keep_cap / 2);
+                crossed = (idx >> 8) != (after >> 8) && after >= q->topk && (q->route == XGM_ROUTE_OR || after >= p.keep_cap / 2);
             } else if (idx < st->pool_cap) {
                 const size_t o = (size_t)st->pool_off + idx;
                 p.pool_w[o] = w; p.pool_d[o] = d; p.pool_k[o] = kv;
@@ -962,7 +867,7 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, 4) xgm_and_bm3_kernel(const __
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
     const uint32_t stage_base = smem_u32(ws.dstage[0]);
     const uint32_t bar_base = stage_base + (uint32_t)offsetof(Bm3Scratch, dbar);
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + 4) == 0) return;
+    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return;
     const uint32_t nitems_bm = p.nitems_bm_dev ? __ldg(p.nitems_bm_dev) : p.nitems_bm;
     uint32_t qn1 = 0, qn2 = 0; /* warp-uniform queue lengths */
     bool done = false;
@@ -1064,7 +969,7 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, 4) xgm_and_bm3_kernel(const __
         /* ---- next work item ---- */
         if (item_end) {
             uint32_t item = 0;
-            if (lane == 0) item = atomicAdd(p.work_counter + 6 + p.pass, 1u);
+            if (lane == 0) item = atomicAdd(p.work_counter + XGM_WC_AND_BM + p.pass, 1u);
             item = __shfl_sync(FULL, item, 0);
             if (item >= nitems_bm) { done = true; continue; }
             const XgmWorkItem wi = p.items_bm[item];
@@ -1220,22 +1125,22 @@ __global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(XgmKernelParams p
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     OrScratch& os = scratch[warp];
     WarpScratch& ws = os.w;
-    if (lane == 0) { mbar_init(&ws.bar, 1); mbar_init(&ws.dbar[0], 1); mbar_init(&ws.dbar[1], 1); }
+    if (lane == 0) mbar_init(&ws.bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
     uint32_t phase = 0;
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
 
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + 4) == 0) return;
+    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return;
     for (;;) {
         uint32_t item = 0;
-        if (lane == 0) item = atomicAdd(p.work_counter + 1 + 2 * p.pass, 1u);
+        if (lane == 0) item = atomicAdd(p.work_counter + XGM_WC_OR + p.pass, 1u);
         item = __shfl_sync(FULL, item, 0);
         if (item >= p.nitems_or) break;
         const XgmWorkItem wi = p.items_or[item];
         if (p.pass != 0 && p.qstate[wi.query].rerun == 0) continue;
         const XgmDevQuery* q = &p.queries[wi.query];
-        if (q->or_fast != 0) continue; /* answered by xgm_or3_kernel */
+        if (q->or_fast != XGM_OR_FAST_GENERAL) continue; /* answered by xgm_or3_kernel */
         const uint32_t nterms = q->nterms;
         const uint32_t drv = wi.pad; /* driver leaf (position in ascending-termfreq order) */
         uint32_t my_begin = 0, my_nblk = 0, my_cur = 0;
@@ -1358,37 +1263,21 @@ __global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(XgmKernelParams p
                 if ((owned & ~skip) >> k & 1u) {
                     const uint32_t d = c[k];
                     const uint32_t dlen = __ldg(&p.doclen[d]);
-                    double stk[XGM_DEV_MAX_TERMS];
-                    uint32_t has = 0; /* bit s: stack slot s holds a value */
-                    int sp = 0;
-                    for (uint32_t i = 0; i < q->prog_len; ++i) {
-                        const int op = q->prog[i];
-                        if (op >= 0) {
-                            if (present[k] >> op & 1u) {
-                                uint32_t tf;
-                                if ((uint32_t)op == drv) {
-                                    tf = unpack_gl(p.tfs, dh.tf_off, 4 * lane + k, XGM_HDR_TF_BITS(dh.meta));
-                                } else if (q->terms[op].bm_off != XGM_NO_BITMAP) {
-                                    const uint32_t r = bitmap_rank(p, q->terms[op], d);
-                                    const XgmBlockHdr bh = hdr[q->terms[op].blk_begin + (r >> 7)];
-                                    tf = unpack_gl(p.tfs, bh.tf_off, r & 127u, XGM_HDR_TF_BITS(bh.meta));
-                                } else {
-                                    tf = os.tft[op][4 * lane + k];
-                                }
-                                stk[sp] = bm25_sumpart(q->terms[op].termweight, q, tf, dlen);
-                                has |= 1u << sp;
-                            } else {
-                                has &= ~(1u << sp);
-                            }
-                            ++sp;
+                    acc[k] = or_tree_weight(q, [&](uint32_t op, double& v) {
+                        if (!(present[k] >> op & 1u)) return false;
+                        uint32_t tf;
+                        if (op == drv) {
+                            tf = unpack_gl(p.tfs, dh.tf_off, 4 * lane + k, XGM_HDR_TF_BITS(dh.meta));
+                        } else if (q->terms[op].bm_off != XGM_NO_BITMAP) {
+                            const uint32_t r = bitmap_rank(p, q->terms[op], d);
+                            const XgmBlockHdr bh = hdr[q->terms[op].blk_begin + (r >> 7)];
+                            tf = unpack_gl(p.tfs, bh.tf_off, r & 127u, XGM_HDR_TF_BITS(bh.meta));
                         } else {
-                            --sp;
-                            const bool hl = has >> (sp - 1) & 1u, hr = has >> sp & 1u;
-                            if (hl && hr) stk[sp - 1] = __dadd_rn(stk[sp - 1], stk[sp]);
-                            else if (hr) { stk[sp - 1] = stk[sp]; has |= 1u << (sp - 1); }
+                            tf = os.tft[op][4 * lane + k];
                         }
-                    }
-                    acc[k] = stk[0];
+                        v = bm25_sumpart(q->terms[op].termweight, q, tf, dlen);
+                        return true;
+                    });
                     aux[k] = __popc(present[k]);
                 }
             }
@@ -1471,11 +1360,11 @@ struct __align__(16) Or3Scratch {
     uint64_t dbar[4];
 };
 
-/* PHASE 0: the whole union in one launch (queries with or_fast == 1).  PHASE 1: the documents holding exactly ONE
- * leaf of the queries whose documents with two or more leaves were already produced by xgm_or_tile_kernel
- * (or_fast == 2) — see there. */
-template <int MINB, int PHASE>
-__global__ void __launch_bounds__(OR3_WARPS * 32, MINB) xgm_or3_kernel(const __grid_constant__ XgmKernelParams p) {
+/* PHASE 0: the whole union in one launch (queries with or_fast == XGM_OR_FAST_OR3).  PHASE 1: the documents holding
+ * exactly ONE leaf of the queries whose documents with two or more leaves were already produced by
+ * xgm_or_tile_kernel (or_fast == XGM_OR_FAST_TILE) — see there. */
+template <int PHASE>
+__global__ void __launch_bounds__(OR3_WARPS * 32, 3) xgm_or3_kernel(const __grid_constant__ XgmKernelParams p) {
     extern __shared__ __align__(16) unsigned char or3_raw[];
     Or3Scratch* scratch = reinterpret_cast<Or3Scratch*>(or3_raw);
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
@@ -1487,7 +1376,7 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, MINB) xgm_or3_kernel(const __g
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
     const uint32_t stage_base = smem_u32(ws.dstage[0]);
     const uint32_t bar_base = stage_base + (uint32_t)offsetof(Or3Scratch, dbar);
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + 4) == 0) return;
+    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return;
     uint32_t qn = 0; /* warp-uniform queue length */
     bool done = false;
     /* current work item: blocks [db, it_b1) of leaf it_drv of query it_query are left */
@@ -1553,13 +1442,13 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, MINB) xgm_or3_kernel(const __g
                 total_acc = 0; it_b1 = 0; db = 0;
             }
             uint32_t item = 0;
-            if (lane == 0) item = atomicAdd(p.work_counter + (PHASE ? 14 : 10) + p.pass, 1u);
+            if (lane == 0) item = atomicAdd(p.work_counter + (PHASE ? XGM_WC_OR3_SINGLE : XGM_WC_OR3) + p.pass, 1u);
             item = __shfl_sync(FULL, item, 0);
             if (item >= p.nitems_or) { done = true; continue; }
             const XgmWorkItem wi = p.items_or[item];
             if (p.pass != 0 && p.qstate[wi.query].rerun == 0) continue;
             q = &p.queries[wi.query];
-            if (q->or_fast != (PHASE ? 2u : 1u)) continue; /* another kernel's query */
+            if (q->or_fast != (PHASE ? XGM_OR_FAST_TILE : XGM_OR_FAST_OR3)) continue; /* another kernel's query */
             nterms = q->nterms;
             it_drv = wi.pad;
             can_prune = (q->sort_by == 0) && (q->topk != 0);
@@ -1684,8 +1573,8 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, MINB) xgm_or3_kernel(const __g
 }
 
 cudaError_t xgm_launch_or3(const XgmKernelParams& p, int grid, int phase, cudaStream_t s) {
-    if (phase) xgm_or3_kernel<3, 1><<<grid, OR3_WARPS * 32, sizeof(Or3Scratch) * OR3_WARPS, s>>>(p);
-    else xgm_or3_kernel<3, 0><<<grid, OR3_WARPS * 32, sizeof(Or3Scratch) * OR3_WARPS, s>>>(p);
+    if (phase) xgm_or3_kernel<1><<<grid, OR3_WARPS * 32, sizeof(Or3Scratch) * OR3_WARPS, s>>>(p);
+    else xgm_or3_kernel<0><<<grid, OR3_WARPS * 32, sizeof(Or3Scratch) * OR3_WARPS, s>>>(p);
     return cudaGetLastError();
 }
 
@@ -1693,9 +1582,9 @@ cudaError_t xgm_launch_or3(const XgmKernelParams& p, int grid, int phase, cudaSt
 int xgm_or3_occupancy_blocks_per_sm() {
     int n = 0;
     const size_t smem = sizeof(Or3Scratch) * OR3_WARPS;
-    cudaFuncSetAttribute(xgm_or3_kernel<3, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(xgm_or3_kernel<3, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_or3_kernel<3, 0>, OR3_WARPS * 32, smem);
+    cudaFuncSetAttribute(xgm_or3_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(xgm_or3_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_or3_kernel<0>, OR3_WARPS * 32, smem);
     return n;
 }
 
@@ -1726,7 +1615,7 @@ __global__ void __launch_bounds__(TILE_WARPS * 32, 4) xgm_or_tile_kernel(const _
     __shared__ TileScratch scratch[TILE_WARPS];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     TileScratch& ws = scratch[warp];
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + 4) == 0) return;
+    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return;
     const uint32_t nwords = (p.lastdocid >> 5) + 1u;
     const uint32_t items_per_q = (nwords + 32u * TILE_ITERS - 1u) / (32u * TILE_ITERS);
     const uint32_t nitems = items_per_q * p.ntileq;
@@ -1746,7 +1635,7 @@ __global__ void __launch_bounds__(TILE_WARPS * 32, 4) xgm_or_tile_kernel(const _
 
     for (;;) {
         uint32_t item = 0;
-        if (lane == 0) item = atomicAdd(p.work_counter + 12 + p.pass, 1u);
+        if (lane == 0) item = atomicAdd(p.work_counter + XGM_WC_TILE + p.pass, 1u);
         item = __shfl_sync(FULL, item, 0);
         if (item >= nitems) break;
         const uint32_t tile = item / p.ntileq, qi = __ldg(p.tileq + (item - tile * p.ntileq));
@@ -2018,18 +1907,18 @@ __device__ __forceinline__ void topk_one_query(const XgmKernelParams& p, const u
                 XgmDevResult r;
                 r.n = 0; r.exact = st.total; r.known = 0; r.max_w = __longlong_as_double((long long)st.maxw);
                 r.max_subqs = q->nweighted; r.pad = 0;
-                /* 64-bit reservation counter (words 8, 9): the sum over a batch of tie-mass queries cannot wrap */
-                const unsigned long long off = atomicAdd(reinterpret_cast<unsigned long long*>(p.work_counter + 8), (unsigned long long)cum);
+                /* 64-bit reservation counter: the sum over a batch of tie-mass queries cannot wrap */
+                const unsigned long long off = atomicAdd(reinterpret_cast<unsigned long long*>(p.work_counter + XGM_WC_POOL), (unsigned long long)cum);
                 if (cum >= topk && off + cum <= (unsigned long long)p.pool_total) {
                     p.qstate[qi].bstar = b;
                     p.qstate[qi].stored = 0;
                     p.qstate[qi].pool_off = (uint32_t)off;
                     p.qstate[qi].pool_cap = cum;
                     p.qstate[qi].rerun = 1;
-                    atomicAdd(p.work_counter + 4, 1u);
-                    r.flags = 4u; /* pending second pass */
+                    atomicAdd(p.work_counter + XGM_WC_RERUN, 1u);
+                    r.flags = XGM_RES_PENDING;
                 } else {
-                    r.flags = 1u; /* overflow pool exhausted */
+                    r.flags = XGM_RES_LOST; /* overflow pool exhausted */
                 }
                 p.out_info[qi] = r;
             }
@@ -2410,7 +2299,7 @@ __device__ __forceinline__ void topk_one_query(const XgmKernelParams& p, const u
         r.n = n < topk ? n : topk;
         r.exact = st.total;
         r.flags = 0;
-        if (kept > p.keep_cap || lost) r.flags |= 1u;
+        if (kept > p.keep_cap || lost) r.flags |= XGM_RES_LOST;
         if (topk == 0) {
             r.known = st.total; /* nothing is ever kept, so min_weight never rises: every match is counted */
         } else if (complete && !st.skipped) {
@@ -2419,10 +2308,10 @@ __device__ __forceinline__ void topk_one_query(const XgmKernelParams& p, const u
             /* pruned run: ProtoMSet's count depends on docid-order history we did not keep; report the
              * guaranteed part and flag the bounds as approximate */
             r.known = st.total < free_count ? st.total : free_count;
-            r.flags |= 2u;
+            r.flags |= XGM_RES_APPROX;
         }
-        if (st.skipped) r.flags |= 8u; /* whole work items were pruned: the match count is a lower bound */
-        if (p.pass != 0) r.flags |= 16u; /* produced by the second pass */
+        if (st.skipped) r.flags |= XGM_RES_SKIPPED;
+        if (p.pass != 0) r.flags |= XGM_RES_SECOND_PASS;
         r.max_w = __longlong_as_double((long long)st.maxw);
         r.max_subqs = q->nweighted;
         r.pad = 0;
@@ -2434,7 +2323,7 @@ __device__ __forceinline__ void topk_one_query(const XgmKernelParams& p, const u
  * BASELINE's C2 queries match <= 32 documents) — do not need a CTA, 45 KB of shared memory and a dozen barriers:
  * one warp ranks up to 64 unpruned relevance-ordered matches (two per lane, pair test against a 768-byte
  * staging area) and every one of them is counted (n <= max(check_at_least, topk + 1): protomset.h:340-376).
- * Everything else is put on topk_list for xgm_topk_kernel (work_counter[16] entries from the front, [19] from the back). */
+ * Everything else is put on topk_list for xgm_topk_kernel (XGM_WC_TOPK_FRONT entries from the front, XGM_WC_TOPK_BACK from the back). */
 #define TOPK_SMALL_WARPS 8
 #define TOPK_SMALL_MAX 64u
 __global__ void __launch_bounds__(TOPK_SMALL_WARPS * 32) xgm_topk_small_kernel(const __grid_constant__ XgmKernelParams p) {
@@ -2453,8 +2342,8 @@ __global__ void __launch_bounds__(TOPK_SMALL_WARPS * 32) xgm_topk_small_kernel(c
         /* longest first: the queries whose exact count needs the sorts (more than 256 stored matches) fill the
          * list from the front, the others from the back, and the CTAs take the front first */
         if (lane == 0) {
-            if (n > TOPK_THREADS) p.topk_list[atomicAdd(p.work_counter + 16, 1u)] = qi;
-            else p.topk_list[p.nq - 1u - atomicAdd(p.work_counter + 19, 1u)] = qi;
+            if (n > TOPK_THREADS) p.topk_list[atomicAdd(p.work_counter + XGM_WC_TOPK_FRONT, 1u)] = qi;
+            else p.topk_list[p.nq - 1u - atomicAdd(p.work_counter + XGM_WC_TOPK_BACK, 1u)] = qi;
         }
         return;
     }
@@ -2506,13 +2395,13 @@ __global__ void __launch_bounds__(TOPK_SMALL_WARPS * 32) xgm_topk_small_kernel(c
  * queries of the batch (no list; second pass) from a counter. */
 __global__ void __launch_bounds__(TOPK_THREADS) xgm_topk_kernel(XgmKernelParams p) {
     __shared__ uint32_t s_slot;
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + 4) == 0) return; /* nothing to re-run */
+    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return; /* nothing to re-run */
     const bool listed = p.topk_list != nullptr && p.pass == 0;
-    const uint32_t nfront = listed ? *reinterpret_cast<volatile uint32_t*>(p.work_counter + 16) : p.nq;
-    const uint32_t count = nfront + (listed ? *reinterpret_cast<volatile uint32_t*>(p.work_counter + 19) : 0u);
+    const uint32_t nfront = listed ? *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_TOPK_FRONT) : p.nq;
+    const uint32_t count = nfront + (listed ? *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_TOPK_BACK) : 0u);
     for (;;) {
         __syncthreads(); /* the previous query's shared state is no longer read */
-        if (threadIdx.x == 0) s_slot = atomicAdd(p.work_counter + 17 + p.pass, 1u);
+        if (threadIdx.x == 0) s_slot = atomicAdd(p.work_counter + XGM_WC_TOPK + p.pass, 1u);
         __syncthreads();
         const uint32_t slot = s_slot;
         if (slot >= count) break;
@@ -2630,42 +2519,28 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32) xgm_decode_kernel(XgmKernelP
 
 /* ------------------------------------------------------------------ work-list expansion */
 
-/* The host only sends one segment per (query[, leaf]): {query, #blocks, first item index, leaf}, and
- * this kernel expands them into work items of `bpi` blocks, in one of two orders:
- *  - level order (AND lists; segments sorted by descending length, level_start[k] = number of items in
- *    levels < k): all queries' first items, then all second items, ...  The warps in flight at any
- *    moment belong to many queries, so every query's pruning threshold rises early, long queries do not
- *    form a tail, and concurrently running items of one query stay far apart;
- *  - segment order (OR list, nlevels == 0): rarest leaves of all queries first, for MaxScore. */
-__global__ void xgm_expand_items_kernel(const XgmWorkItem* __restrict__ seg, uint32_t nseg, uint32_t total,
+/* The host only sends one segment per (query[, leaf]): {query, #blocks, 0, leaf}, sorted by descending #blocks,
+ * and this kernel expands them into work items of `bpi` blocks in level order (level_start[k] = number of items in
+ * levels < k, nlevels >= 1): all queries' first items, then all second items, ...  The warps in flight at any
+ * moment belong to many queries, so every query's pruning threshold rises early, long queries do not form a tail,
+ * and concurrently running items of one query stay far apart.  The OR list is expanded one leaf group at a time,
+ * rarest leaves of all queries first, for MaxScore.  The range-major bitmap AND list has its own kernels below. */
+__global__ void xgm_expand_items_kernel(const XgmWorkItem* __restrict__ seg, uint32_t total,
                                         const uint32_t* __restrict__ level_start, uint32_t nlevels, uint32_t bpi,
                                         XgmWorkItem* __restrict__ out) {
     const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= total) return;
-    XgmWorkItem w;
-    if (nlevels != 0) {
-        uint32_t lo = 0, hi = nlevels; /* last level whose start is <= s */
-        while (hi - lo > 1) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (level_start[mid] <= s) lo = mid; else hi = mid;
-        }
-        const XgmWorkItem sg = seg[s - level_start[lo]]; /* segments sorted by descending #blocks */
-        w.query = sg.query;
-        w.b0 = lo * bpi;
-        w.b1 = min(sg.b0, w.b0 + bpi);
-        w.pad = sg.pad;
-    } else {
-        uint32_t lo = 0, hi = nseg; /* last segment whose first item index (field b1) is <= s */
-        while (hi - lo > 1) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (seg[mid].b1 <= s) lo = mid; else hi = mid;
-        }
-        const XgmWorkItem sg = seg[lo]; /* query, b0 = #blocks, b1 = first item index, pad = leaf */
-        w.query = sg.query;
-        w.b0 = (s - sg.b1) * bpi;
-        w.b1 = min(sg.b0, w.b0 + bpi);
-        w.pad = sg.pad;
+    uint32_t lo = 0, hi = nlevels; /* last level whose start is <= s */
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (level_start[mid] <= s) lo = mid; else hi = mid;
     }
+    const XgmWorkItem sg = seg[s - level_start[lo]];
+    XgmWorkItem w;
+    w.query = sg.query;
+    w.b0 = lo * bpi;
+    w.b1 = min(sg.b0, w.b0 + bpi);
+    w.pad = sg.pad;
     out[s] = w;
 }
 
@@ -2793,10 +2668,10 @@ cudaError_t xgm_launch_expand_ranges(const XgmWorkItem* runs, uint32_t nruns, co
     return cudaGetLastError();
 }
 
-cudaError_t xgm_launch_expand(const XgmWorkItem* seg, uint32_t nseg, uint32_t total, const uint32_t* level_start,
-                              uint32_t nlevels, uint32_t bpi, XgmWorkItem* out, cudaStream_t s) {
+cudaError_t xgm_launch_expand(const XgmWorkItem* seg, uint32_t total, const uint32_t* level_start, uint32_t nlevels,
+                              uint32_t bpi, XgmWorkItem* out, cudaStream_t s) {
     if (total == 0) return cudaSuccess;
-    xgm_expand_items_kernel<<<(total + 255) / 256, 256, 0, s>>>(seg, nseg, total, level_start, nlevels, bpi, out);
+    xgm_expand_items_kernel<<<(total + 255) / 256, 256, 0, s>>>(seg, total, level_start, nlevels, bpi, out);
     return cudaGetLastError();
 }
 
