@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <cfloat>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -904,7 +905,7 @@ struct PlannedQuery {
     bool on_device = false;   /* false: answered on the host (empty / bounds-only) */
     uint32_t first = 0, maxitems = 0, topk = 0, check_at_least = 0;
     uint32_t tf_min = 0, tf_est = 0, tf_max = 0;
-    uint32_t nterms = 0;
+    uint32_t nweighted = 0;   /* weighted subqueries: the denominator of the percentage scale */
     double max_possible = 0;
     uint64_t alg_bytes = 0;
     uint32_t sort_by = 0;
@@ -1055,6 +1056,7 @@ struct xgm_searcher {
     bool device_only = false;     /* results stay on the device (xgm_searcher_set_results_on_device) */
     uint32_t bpi_override = 0;    /* XGM_BPI: driver blocks per work item for batches >= 256 (default 16) */
     bool or_tile = true;          /* XGM_OR_TILE=0: keep every fast OR query in the one-launch kernel */
+    bool or_general = false;      /* XGM_OR_KERNEL=1: every OR query on the general xgm_or_kernel */
     XgmKernelParams params;
     /* xgm_search_submit_async: a worker thread plans and enqueues the batch while the caller scatters the
      * results of an earlier one */
@@ -1158,6 +1160,7 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
     CUDA_TRY(cudaMallocHost(&s->h_tileq, nq * 4));
     CUDA_TRY(cudaMalloc(&s->d_tileq, nq * 4));
     if (const char* e = getenv("XGM_OR_TILE")) s->or_tile = atoi(e) != 0;
+    if (const char* e = getenv("XGM_OR_KERNEL")) s->or_general = atoi(e) == 1;
     if (const char* e = getenv("XGM_BPI")) s->bpi_override = (uint32_t)std::min(32, std::max(0, atoi(e)));
     CUDA_TRY(cudaMalloc(&s->d_raise, nq * XGM_RAISE_LOG * sizeof(XgmRaise)));
     s->ctrl_bytes = XGM_CTRL_HDR + nq * sizeof(XgmQState) + nq * XGM_NBINS * 4;
@@ -1208,6 +1211,7 @@ extern "C" void* xgm_searcher_stream(xgm_searcher* s) { return s ? (void*)s->str
 /* ComparePostListTermFreqAscending on (tf, original index) — same std::partial_sort_copy call as
  * MultiAndPostList's constructor (multiandpostlist.h:126-131) so ties land identically (libstdc++). */
 struct TfIdx { uint32_t tf, idx; };
+static inline bool tf_less(const TfIdx& a, const TfIdx& c) { return a.tf < c.tf; }
 
 /* Heap::make/pop/replace of src/xapian/common/heap.h (libc++-style sift-down) replayed on
  * (termfreq, node) pairs exactly as OrContext::postlist does (queryinternal.cc:440-489). */
@@ -1254,30 +1258,64 @@ static void build_or_tree(const uint32_t* tf, uint32_t n, OrTree& tr) {
     }
 }
 
-/* Termfreq (min, max, estimate) of an OrContext::postlist tree over leaves with termfreqs tf[]:
- * OrPostList::get_termfreq_min/max/est (matcher/orpostlist.cc:80-83,353-384) folded bottom-up. */
+/* Termfreq (min, max, estimate) of a PostList */
 struct TfNode { uint32_t mn, mx, est; };
-static TfNode or_group_node(const uint32_t* tf, uint32_t n, uint32_t doccount) {
-    TfNode out{0, 0, 0};
-    if (n == 0) return out;
-    if (n == 1) return TfNode{tf[0], tf[0], tf[0]};
-    OrTree tr;
-    build_or_tree(tf, n, tr);
-    TfNode val[2 * XGM_MAX_TERMS];
-    for (uint32_t i = 0; i < n; ++i) val[i] = TfNode{tf[i], tf[i], tf[i]};
-    const double dbsize = doccount;
-    for (int node = (int)n; node <= tr.root; ++node) { /* internal nodes are created children-first */
-        const TfNode l = val[tr.lch[node]], r = val[tr.rch[node]];
-        TfNode v;
-        v.mn = std::max(l.mn, r.mn);
-        uint32_t t = l.mx + r.mx;
-        if (t > doccount || t < l.mx) t = doccount;
-        v.mx = t;
-        const double a = l.est, b = r.est;
-        v.est = dbsize == 0.0 ? 0 : (uint32_t)(a + b - (a * b / dbsize) + 0.5);
-        val[node] = v;
+
+/* MultiAndPostList::get_termfreq_{min,max,est} (matcher/multiandpostlist.cc:55-105) over the children ch[0 .. n) in
+ * the order given: the wrapping sum of the minimums, the least maximum and the scaled product of the estimates */
+static TfNode and_node(const TfNode* ch, uint32_t n, uint32_t doccount) {
+    uint32_t sum = ch[0].mn;
+    if (sum) {
+        for (uint32_t i = 1; i < n; ++i) {
+            const uint32_t old = sum;
+            sum += ch[i].mn;
+            if (sum >= old && sum <= doccount) { sum = 0; break; }
+            sum -= doccount;
+        }
     }
-    return val[tr.root];
+    const double dbsize = doccount;
+    uint32_t mx = ch[0].mx;
+    double r = ch[0].est;
+    for (uint32_t i = 1; i < n; ++i) {
+        mx = std::min(mx, ch[i].mx);
+        r = (r * ch[i].est) / dbsize;
+    }
+    return TfNode{sum, mx, doccount ? (uint32_t)(r + 0.5) : 0};
+}
+
+static void or_postfix(const OrTree& tr, int x, uint32_t n, const uint32_t* label, XgmDevQuery& dq) {
+    if (x < (int)n) { dq.prog[dq.prog_len++] = (int8_t)(label ? label[x] : (uint32_t)x); return; }
+    or_postfix(tr, tr.lch[x], n, label, dq);
+    or_postfix(tr, tr.rch[x], n, label, dq);
+    dq.prog[dq.prog_len++] = -1;
+}
+
+/* The OrContext::postlist tree over leaves with termfreqs tf[0 .. n) and max weights w[] (none: 0), folded
+ * bottom-up: termfreqs by OrPostList::get_termfreq_min/max/est (matcher/orpostlist.cc:80-83,353-384), max weight
+ * left + right (OrPostList::recalc_maxweight, orpostlist.cc:105-111).  With dq, the tree also becomes dq->prog,
+ * the device's postfix program: left subtree, right subtree, -1, with leaf i written as label[i] (i without labels). */
+struct OrFold { TfNode tf; double maxw; };
+static OrFold or_fold(const uint32_t* tf, const double* w, uint32_t n, uint32_t doccount,
+                      const uint32_t* label = nullptr, XgmDevQuery* dq = nullptr) {
+    OrTree tr;
+    tr.root = 0; /* a single leaf is the whole tree */
+    if (n > 1) build_or_tree(tf, n, tr);
+    OrFold v[2 * XGM_MAX_TERMS];
+    for (uint32_t i = 0; i < n; ++i) v[i] = OrFold{TfNode{tf[i], tf[i], tf[i]}, w ? w[i] : 0.0};
+    const double dbsize = doccount;
+    for (int x = (int)n; x <= tr.root; ++x) { /* internal nodes are created children-first */
+        const OrFold l = v[tr.lch[x]], r = v[tr.rch[x]];
+        uint32_t mx = l.tf.mx + r.tf.mx;
+        if (mx > doccount || mx < l.tf.mx) mx = doccount;
+        const double a = l.tf.est, b = r.tf.est;
+        const uint32_t est = dbsize == 0.0 ? 0 : (uint32_t)(a + b - (a * b / dbsize) + 0.5);
+        v[x] = OrFold{TfNode{std::max(l.tf.mn, r.tf.mn), mx, est}, l.maxw + r.maxw};
+    }
+    if (dq) {
+        dq->prog_len = 0;
+        or_postfix(tr, tr.root, n, label, *dq);
+    }
+    return v[tr.root];
 }
 
 /* BM25Weight::init (bm25weight.cc:46-130) via Weight::init_ (weight.cc:59-83); host-side because it
@@ -1308,57 +1346,266 @@ static double bm25_maxpart(double termweight, double len_factor, double k1, doub
     return termweight * (wdf_max / denom);
 }
 
-static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, PlannedQuery& pq, XgmDevQuery& dq,
-                             PlannedSegments& segs) {
-    const xgm_index* ix = s->ix;
-    pq = PlannedQuery();
-    memset(&dq, 0, offsetof(XgmDevQuery, terms)); /* the term slots in use are written in full by put_term */
-    if (q.nterms == 0 || q.nterms > XGM_MAX_TERMS) { pq.status = XGM_E_UNIMPLEMENTED; return XGM_OK; }
-    if (q.op != XGM_OP_AND && q.op != XGM_OP_OR) { pq.status = XGM_E_UNIMPLEMENTED; return XGM_OK; }
-    const uint32_t nfilter = q.nfilter, nnot = q.nnot, nmaybe = q.nmaybe, ngroups = q.nfilter + q.nnot + q.nmaybe;
-    if (ngroups) {
+/* A query's leaves as the planner sees them: the nterms base terms, then the FILTER, AND_NOT and AND_MAYBE groups */
+struct PlanTerms {
+    uint32_t n, nfilter, nnot, nmaybe, ngroups;
+    uint32_t ids[XGM_MAX_TERMS]; /* 0xffffffffu: not in this index */
+    uint32_t ltf[XGM_MAX_TERMS]; /* termfreq in this index (0 if absent) */
+    /* BM25 parameters and the base terms' weights */
+    uint32_t N;
+    double k1, k3, b, mnl, len_factor;
+    double tw[XGM_MAX_TERMS], maxpart[XGM_MAX_TERMS];
+    uint32_t nweighted; /* base terms with a nonzero factor */
+};
+
+/* Checks the query's shape and arguments and looks up its leaves.  Anything but XGM_OK declines the query. */
+static xgm_status resolve_terms(const xgm_index* ix, const xgm_query& q, PlanTerms& t) {
+    if (q.nterms == 0 || q.nterms > XGM_MAX_TERMS) return XGM_E_UNIMPLEMENTED;
+    if (q.op != XGM_OP_AND && q.op != XGM_OP_OR) return XGM_E_UNIMPLEMENTED;
+    const bool groups = q.nfilter || q.nnot || q.nmaybe;
+    if (groups) {
         /* OP_FILTER with boolean terms / OP_AND_NOT / OP_AND_MAYBE around an AND (or single-term) base, the first
          * two also around an OR base; optional leaves on an OR base or a value-range filter on top are left to the
          * reference */
         const bool or_base = q.op == XGM_OP_OR && q.nterms != 1;
         if ((or_base && q.nmaybe) || q.filter != XGM_FILTER_NONE ||
-            (uint64_t)q.nterms + ngroups > XGM_MAX_TERMS) {
-            pq.status = XGM_E_UNIMPLEMENTED;
-            return XGM_OK;
-        }
+            (uint64_t)q.nterms + q.nfilter + q.nnot + q.nmaybe > XGM_MAX_TERMS)
+            return XGM_E_UNIMPLEMENTED;
     }
-    if (q.sort_by > XGM_SORT_REL_VAL || q.filter > XGM_FILTER_MULTI_RANGE) { pq.status = XGM_E_INVALID; return XGM_OK; }
-    if ((q.filter && q.filter_slot >= XGM_MAX_SLOTS) || (q.sort_by && q.sort_slot >= XGM_MAX_SLOTS)) { pq.status = XGM_E_INVALID; return XGM_OK; }
-    if (q.revision != 0 && q.revision != ix->revision) { pq.status = XGM_E_STALE; return XGM_OK; }
+    if (q.sort_by > XGM_SORT_REL_VAL || q.filter > XGM_FILTER_MULTI_RANGE) return XGM_E_INVALID;
+    if ((q.filter && q.filter_slot >= XGM_MAX_SLOTS) || (q.sort_by && q.sort_slot >= XGM_MAX_SLOTS)) return XGM_E_INVALID;
+    if (q.revision != 0 && q.revision != ix->revision) return XGM_E_STALE;
     if ((q.filter && !ix->slot_exact[q.filter_slot] && ix->d_voff[q.filter_slot]) ||
-        (q.sort_by && !ix->slot_exact[q.sort_slot] && ix->d_voff[q.sort_slot])) {
-        pq.status = XGM_E_UNIMPLEMENTED; /* values longer than 8 bytes: their keys do not decide the comparison */
-        return XGM_OK;
-    }
-    /* the source of a Xapiand range (MultipleValueRange) takes part in the MultiAndPostList like a term with
-     * termfreq (min, est, max) = (0, value_freq, value_freq) (range.cc:457-464, api/postingsource.cc:201-214) */
-    const bool mv_source = q.filter == XGM_FILTER_MULTI_RANGE;
-    const bool src_weighted = mv_source && q.filter_weighted;
-    if (q.filter_weighted && (!mv_source || (q.op != XGM_OP_AND && q.nterms != 1) || ngroups)) { pq.status = XGM_E_UNIMPLEMENTED; return XGM_OK; }
-    const double src_w = src_weighted ? (q.filter_factor != 0.0 ? q.filter_factor : 1.0) * 1.0 : 0.0;
-    if (src_w < 0.0) { pq.status = XGM_E_UNIMPLEMENTED; return XGM_OK; }
-    const uint32_t n = q.nterms;
-    const uint32_t nall = n + ngroups; /* base terms, then filter terms, then excluded terms */
-    uint32_t ids[XGM_MAX_TERMS];
-    uint32_t ltf[XGM_MAX_TERMS];
-    for (uint32_t j = 0; j < nall; ++j) {
+        (q.sort_by && !ix->slot_exact[q.sort_slot] && ix->d_voff[q.sort_slot]))
+        return XGM_E_UNIMPLEMENTED; /* values longer than 8 bytes: their keys do not decide the comparison */
+    /* a weighted range source: a child of the AND (or of a single term) without groups, with a factor >= 0 */
+    if (q.filter_weighted && (q.filter != XGM_FILTER_MULTI_RANGE || (q.op != XGM_OP_AND && q.nterms != 1) || groups ||
+                              q.filter_factor < 0.0))
+        return XGM_E_UNIMPLEMENTED;
+    t.n = q.nterms; t.nfilter = q.nfilter; t.nnot = q.nnot; t.nmaybe = q.nmaybe;
+    t.ngroups = q.nfilter + q.nnot + q.nmaybe;
+    for (uint32_t j = 0; j < t.n + t.ngroups; ++j) {
         uint32_t id = 0xffffffffu;
         if (q.term_ids) id = q.term_ids[j];
         else if (q.terms && q.terms[j]) {
             uint32_t len = q.term_lens ? q.term_lens[j] : (uint32_t)strlen(q.terms[j]);
             if (!lookup_term(ix, q.terms[j], len, &id)) id = 0xffffffffu;
-        } else { pq.status = XGM_E_INVALID; return XGM_OK; }
-        if (id != 0xffffffffu && id >= ix->terms.size()) { pq.status = XGM_E_INVALID; return XGM_OK; }
-        ids[j] = id;
-        ltf[j] = id == 0xffffffffu ? 0 : ix->terms[id].termfreq;
+        } else return XGM_E_INVALID;
+        if (id != 0xffffffffu && id >= ix->terms.size()) return XGM_E_INVALID;
         for (uint32_t i = 0; i < j; ++i)
-            if (ids[i] == id && id != 0xffffffffu) { pq.status = XGM_E_UNIMPLEMENTED; return XGM_OK; } /* repeated leaf */
+            if (t.ids[i] == id && id != 0xffffffffu) return XGM_E_UNIMPLEMENTED; /* repeated leaf */
+        t.ids[j] = id;
+        t.ltf[j] = id == 0xffffffffu ? 0 : ix->terms[id].termfreq;
     }
+    return XGM_OK;
+}
+
+/* Weight::init_ of leaf j: its BM25 termweight and maxpart */
+static void term_weight(const xgm_index* ix, const xgm_query& q, const PlanTerms& t, uint32_t j, double factor,
+                        double& tw, double& maxpart) {
+    const uint32_t gtf = q.stats ? q.stats->termfreq[j] : t.ltf[j];
+    tw = bm25_termweight(t.N, gtf, q.wqf ? q.wqf[j] : 1, factor, t.k1, t.k3);
+    const uint32_t wub = t.ids[j] == 0xffffffffu ? 0 : ix->terms[t.ids[j]].wdf_ub;
+    maxpart = bm25_maxpart(tw, t.len_factor, t.k1, t.b, t.mnl, wub, ix->doclen_lb);
+}
+
+/* The BM25 parameters and the base terms' weights.  A negative factor, or a zero one in an OR of several leaves,
+ * declines the query. */
+static xgm_status weigh_terms(const xgm_index* ix, const xgm_query& q, PlanTerms& t) {
+    t.k1 = q.k1; t.k3 = q.k3; t.b = q.b; t.mnl = q.min_normlen;
+    if (t.k1 == 0 && t.k3 == 0 && t.b == 0 && t.mnl == 0) { t.k1 = 1; t.k3 = 1; t.b = 0.5; t.mnl = 0.5; }
+    t.N = q.stats ? q.stats->collection_size : ix->doccount;
+    const uint64_t tl = q.stats ? q.stats->total_length : ix->total_length;
+    t.len_factor = 0;
+    if (!(t.b == 0 || t.k1 == 0)) {
+        double avg = t.N == 0 ? 0.0 : (double)tl / t.N;
+        t.len_factor = avg != 0 ? 1 / avg : 0;
+    }
+    t.nweighted = 0;
+    for (uint32_t j = 0; j < t.n; ++j) {
+        const double factor = q.factors ? q.factors[j] : 1.0;
+        if (factor < 0.0 || (factor == 0.0 && q.op == XGM_OP_OR && t.n > 1)) return XGM_E_UNIMPLEMENTED;
+        term_weight(ix, q, t, j, factor, t.tw[j], t.maxpart[j]);
+        if (factor == 0.0) { t.tw[j] = 0.0; t.maxpart[j] = 0.0; } /* no Weight object: not a counted subquery */
+        else ++t.nweighted;
+    }
+    return XGM_OK;
+}
+
+/* Device slot of leaf `id` (0xffffffffu: not in this index) with its weight pair.  A boolean leaf has (0.0, 0.0):
+ * it adds +0.0 to the weight sum, which leaves the sum unchanged. */
+static void put_term(const xgm_index* ix, XgmDevTerm& d, uint32_t id, double termweight, double maxpart) {
+    d.termweight = termweight;
+    d.maxpart = maxpart;
+    d.bm_off = XGM_NO_BITMAP; d.rk_off = 0;
+    d.blk_begin = 0; d.nblocks = 0;
+    if (id != 0xffffffffu) {
+        const TermInfo& tinf = ix->terms[id];
+        d.blk_begin = tinf.blk_begin; d.nblocks = tinf.nblocks;
+        d.bm_off = tinf.bm_off; d.rk_off = tinf.rk_off;
+    }
+}
+
+/* The AND_NOT terms from slot on, as boolean leaves: only those in this index (the others exclude nothing).
+ * Returns the next free slot. */
+static uint32_t put_excluded(const xgm_index* ix, const PlanTerms& t, XgmDevQuery& dq, uint32_t slot) {
+    const uint32_t nb = t.n + t.nfilter;
+    for (uint32_t j = nb; j < nb + t.nnot; ++j)
+        if (t.ltf[j] != 0) { put_term(ix, dq.terms[slot++], t.ids[j], 0.0, 0.0); ++dq.nnot; }
+    return slot;
+}
+
+/* Termfreq bounds of the groups around a base with bounds cur: MultiAnd(base, AND of the FILTER terms), then
+ * AndNot(…, OR of the AND_NOT terms).  AND_MAYBE keeps its left side's. */
+static TfNode group_bounds(const xgm_index* ix, const PlanTerms& t, TfNode cur) {
+    const uint32_t doccount = ix->doccount;
+    if (t.nfilter) {
+        /* QueryFilter::postlist: MultiAndPostList of [base, Query(OP_AND, boolean terms)] */
+        const uint32_t* ftf = t.ltf + t.n;
+        TfNode f{ftf[0], ftf[0], ftf[0]};
+        if (t.nfilter > 1) {
+            TfNode fin[XGM_MAX_TERMS], fo[XGM_MAX_TERMS];
+            for (uint32_t j = 0; j < t.nfilter; ++j) fin[j] = TfNode{ftf[j], ftf[j], ftf[j]};
+            std::partial_sort_copy(fin, fin + t.nfilter, fo, fo + t.nfilter,
+                                   [](const TfNode& a, const TfNode& c) { return a.est < c.est; });
+            f = and_node(fo, t.nfilter, doccount);
+        }
+        /* the pair by ascending estimate, the base first on a tie */
+        const TfNode ch[2] = {f.est < cur.est ? f : cur, f.est < cur.est ? cur : f};
+        cur = and_node(ch, 2, doccount);
+    }
+    if (t.nnot) {
+        /* AndNotPostList::get_termfreq_min/max/est, matcher/andnotpostlist.cc:30-62 */
+        const TfNode rr = or_fold(t.ltf + t.n + t.nfilter, nullptr, t.nnot, doccount).tf;
+        const TfNode a = cur;
+        cur.mn = a.mn <= rr.mx ? 0 : a.mn - rr.mx;
+        cur.mx = std::min(doccount - rr.mn, a.mx);
+        if (doccount == 0) cur.est = 0;
+        else {
+            double e = a.est;
+            e = (e * (double)(doccount - rr.est)) / (double)doccount;
+            cur.est = (uint32_t)(e + 0.5);
+        }
+    }
+    return cur;
+}
+
+/* An AND base: one MultiAndPostList over the base terms and, for a Xapiand range, its source; the FILTER terms join
+ * the required lists as boolean leaves, then the AND_NOT and AND_MAYBE terms follow. */
+static void plan_and_route(const xgm_index* ix, const xgm_query& q, const PlanTerms& t, PlannedQuery& pq,
+                           XgmDevQuery& dq) {
+    const uint32_t n = t.n;
+    /* the source of a Xapiand range (MultipleValueRange) takes part in the MultiAndPostList like a term with
+     * termfreq (min, est, max) = (0, value_freq, value_freq) (range.cc:457-464, api/postingsource.cc:201-214) */
+    const bool mv_source = q.filter == XGM_FILTER_MULTI_RANGE;
+    const bool src_weighted = mv_source && q.filter_weighted;
+    const double src_w = src_weighted ? (q.filter_factor != 0.0 ? q.filter_factor : 1.0) : 0.0;
+    /* its children sorted by get_termfreq_est with the very call of multiandpostlist.h:126-131 */
+    const uint32_t nch = n + (mv_source ? 1u : 0u);
+    const uint32_t src_vf = mv_source ? ix->slot_freq[q.filter_slot] : 0u;
+    TfIdx in[XGM_MAX_TERMS + 1], outv[XGM_MAX_TERMS + 1];
+    for (uint32_t j = 0; j < n; ++j) in[j] = TfIdx{t.ltf[j], j};
+    if (mv_source) in[n] = TfIdx{src_vf, n};
+    std::partial_sort_copy(in, in + nch, outv, outv + nch, tf_less);
+    /* MultiAndPostList::recalc_maxweight (multiandpostlist.cc:167-177) and termfreqs over the children in that
+     * order: base term order[i], or the source at src_pos */
+    uint32_t order[XGM_MAX_TERMS], src_pos = XGM_NO_SRC, k = 0;
+    TfNode ch[XGM_MAX_TERMS + 1];
+    double mp = 0, mp_real = 0;
+    for (uint32_t c = 0; c < nch; ++c) {
+        const uint32_t j = outv[c].idx;
+        if (j == n) {
+            src_pos = k;
+            ch[c] = TfNode{0, src_vf, src_vf};
+            mp += src_weighted ? src_w * DBL_MAX : 0.0;
+            mp_real += src_w;
+        } else {
+            order[k++] = j;
+            ch[c] = TfNode{t.ltf[j], t.ltf[j], t.ltf[j]};
+            mp += t.maxpart[j];
+            mp_real += t.maxpart[j];
+        }
+    }
+    pq.max_possible = nch == 1 ? t.maxpart[0] : mp;
+    pq.bucket_max = nch == 1 ? t.maxpart[0] : mp_real;
+    const TfNode cur = group_bounds(ix, t, and_node(ch, nch, ix->doccount));
+    pq.tf_min = cur.mn; pq.tf_max = cur.mx; pq.tf_est = cur.est;
+    pq.mv_source = mv_source;
+    if (src_weighted) { dq.src_pos = src_pos; dq.src_weight = src_w; }
+    dq.route = XGM_ROUTE_AND;
+    dq.nterms = n + t.nfilter;
+    /* required lists: the base (its own MultiAndPostList order, which fixes the order of the weight sum) merged with
+     * the boolean filter terms by ascending termfreq */
+    TfIdx fin[XGM_MAX_TERMS];
+    for (uint32_t j = 0; j < t.nfilter; ++j) fin[j] = TfIdx{t.ltf[n + j], n + j};
+    std::stable_sort(fin, fin + t.nfilter, tf_less);
+    uint32_t slot = 0, bi = 0, fi = 0;
+    while (bi < n || fi < t.nfilter) {
+        if (fi >= t.nfilter || (bi < n && t.ltf[order[bi]] <= fin[fi].tf)) {
+            const uint32_t j = order[bi++];
+            put_term(ix, dq.terms[slot++], t.ids[j], t.tw[j], t.maxpart[j]);
+        } else {
+            put_term(ix, dq.terms[slot++], t.ids[fin[fi++].idx], 0.0, 0.0);
+        }
+    }
+    slot = put_excluded(ix, t, dq, slot);
+    if (t.nmaybe) {
+        /* AndMaybePostList: termfreqs are the left's; recalc_maxweight = pl_max + r_max where r is the
+         * OrContext tree over the optional leaves (matcher/andmaybepostlist.cc:69-75); prog names them in
+         * query order */
+        const uint32_t mb = n + t.nfilter + t.nnot;
+        double mtw[XGM_MAX_TERMS], mmax[XGM_MAX_TERMS];
+        for (uint32_t j = 0; j < t.nmaybe; ++j) term_weight(ix, q, t, mb + j, 1.0, mtw[j], mmax[j]);
+        pq.max_possible = pq.max_possible + or_fold(t.ltf + mb, mmax, t.nmaybe, ix->doccount, nullptr, &dq).maxw;
+        pq.bucket_max = pq.max_possible;
+        for (uint32_t j = 0; j < t.nmaybe; ++j) put_term(ix, dq.terms[slot++], t.ids[mb + j], mtw[j], mmax[j]);
+        dq.nmaybe = t.nmaybe;
+        pq.aux_subqs = true;
+    }
+    /* weighted subqueries, for the percentage scale (a weighted source excludes groups) */
+    pq.nweighted = t.nweighted + (src_weighted ? 1u : 0u) + t.nmaybe;
+}
+
+/* An OR base of several leaves: a Huffman-shaped tree of binary OrPostLists, built from the leaves in query order
+ * (OrContext::postlist, queryinternal.cc:440-489).  On the device the leaves are stored in ascending-termfreq order
+ * (position = ownership priority); the program refers to positions. */
+static void plan_or_route(const xgm_index* ix, const PlanTerms& t, PlannedQuery& pq, XgmDevQuery& dq) {
+    const uint32_t n = t.n;
+    TfIdx in[XGM_MAX_TERMS];
+    for (uint32_t j = 0; j < n; ++j) in[j] = TfIdx{t.ltf[j], j};
+    std::stable_sort(in, in + n, tf_less);
+    uint32_t posof[XGM_MAX_TERMS];
+    for (uint32_t i = 0; i < n; ++i) posof[in[i].idx] = i;
+    const OrFold f = or_fold(t.ltf, t.maxpart, n, ix->doccount, posof, &dq);
+    /* QueryFilter / QueryAndNot above the OrPostList tree: the filter's boolean terms and the excluded terms weigh
+     * nothing (MultiAndPostList::get_weight adds +0.0, AndNotPostList returns the left's weight), so a match keeps
+     * the tree's weight; the counts follow the same bound arithmetic as around an AND base. */
+    const TfNode cur = group_bounds(ix, t, f.tf);
+    pq.tf_min = cur.mn; pq.tf_max = cur.mx; pq.tf_est = cur.est;
+    pq.max_possible = f.maxw;
+    pq.bucket_max = pq.max_possible;
+    pq.nweighted = t.nweighted; /* every leaf: a zero factor was declined */
+    dq.route = XGM_ROUTE_OR;
+    dq.nterms = n;
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t j = in[i].idx;
+        put_term(ix, dq.terms[i], t.ids[j], t.tw[j], t.maxpart[j]);
+    }
+    /* terms[n .. n + or_nreq) must hold the document, terms[n + or_nreq .. + nnot) must not */
+    for (uint32_t j = 0; j < t.nfilter; ++j) put_term(ix, dq.terms[n + j], t.ids[n + j], 0.0, 0.0);
+    dq.or_nreq = t.nfilter;
+    put_excluded(ix, t, dq, n + t.nfilter);
+}
+
+/* Plans query qi of a batch into pq and dq and adds its segments; its outcome is pq.status. */
+static void plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, PlannedQuery& pq, XgmDevQuery& dq,
+                       PlannedSegments& segs) {
+    const xgm_index* ix = s->ix;
+    pq = PlannedQuery();
+    memset(&dq, 0, offsetof(XgmDevQuery, terms)); /* the term slots in use are written in full by put_term */
+    PlanTerms t;
+    pq.status = resolve_terms(ix, q, t);
+    if (pq.status != XGM_OK) return;
     /* Enquire::Internal::get_mset clamping, api/enquire.cc:420-426 */
     uint32_t docs = ix->doccount;
     uint32_t first = std::min(q.first, docs);
@@ -1366,304 +1613,30 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
     uint32_t cal = std::min(q.check_at_least, docs);
     cal = std::max(cal, first + maxitems);
     pq.first = first; pq.maxitems = maxitems; pq.topk = first + maxitems; pq.check_at_least = cal;
-    pq.nterms = n; pq.sort_by = q.sort_by; pq.filter = q.filter;
+    pq.sort_by = q.sort_by; pq.filter = q.filter;
+    pq.status = weigh_terms(ix, q, t);
+    if (pq.status != XGM_OK) return;
 
-    double k1 = q.k1, k3 = q.k3, b = q.b, mnl = q.min_normlen;
-    if (k1 == 0 && k3 == 0 && b == 0 && mnl == 0) { k1 = 1; k3 = 1; b = 0.5; mnl = 0.5; }
-    uint32_t N = q.stats ? q.stats->collection_size : ix->doccount;
-    uint64_t tl = q.stats ? q.stats->total_length : ix->total_length;
-    double len_factor = 0;
-    if (!(b == 0 || k1 == 0)) {
-        double avg = N == 0 ? 0.0 : (double)tl / N;
-        len_factor = avg != 0 ? 1 / avg : 0;
-    }
-    double tw[XGM_MAX_TERMS], maxpart[XGM_MAX_TERMS];
-    uint32_t nweighted_base = 0;
-    for (uint32_t j = 0; j < n; ++j) {
-        uint32_t gtf = q.stats ? q.stats->termfreq[j] : ltf[j];
-        const double factor = q.factors ? q.factors[j] : 1.0;
-        if (factor < 0.0 || (factor == 0.0 && q.op == XGM_OP_OR && n > 1)) { pq.status = XGM_E_UNIMPLEMENTED; return XGM_OK; }
-        tw[j] = bm25_termweight(N, gtf, q.wqf ? q.wqf[j] : 1, factor, k1, k3);
-        uint32_t wub = ids[j] == 0xffffffffu ? 0 : ix->terms[ids[j]].wdf_ub;
-        maxpart[j] = bm25_maxpart(tw[j], len_factor, k1, b, mnl, wub, ix->doclen_lb);
-        if (factor == 0.0) { tw[j] = 0.0; maxpart[j] = 0.0; } /* no Weight object: not a counted subquery */
-        else ++nweighted_base;
-    }
-    dq.op = q.op; dq.nterms = n + nfilter; dq.nweighted = q.op == XGM_OP_OR && n > 1 ? n : nweighted_base;
+    dq.op = q.op; dq.nweighted = t.nweighted;
     dq.topk = pq.topk; dq.check_at_least = cal;
-    pq.nterms = nweighted_base + (src_weighted ? 1u : 0u); /* total weighted subqueries, for the percentage scale */
-    dq.len_factor = len_factor; dq.k1 = k1; dq.b = b; dq.one_minus_b = 1 - b; dq.min_normlen = mnl;
+    dq.len_factor = t.len_factor; dq.k1 = t.k1; dq.b = t.b; dq.one_minus_b = 1 - t.b; dq.min_normlen = t.mnl;
     dq.filter = q.filter; dq.filter_slot = q.filter_slot; dq.range_lo = q.range_lo; dq.range_hi = q.range_hi;
     dq.sort_by = q.sort_by; dq.sort_slot = q.sort_slot; dq.sort_reverse = q.sort_reverse; dq.sort_use_max = q.sort_use_max;
     dq.sort_missing = q.sort_missing_key;
     dq.src_pos = XGM_NO_SRC; dq.src_weight = 0.0;
-    double dbsize = ix->doccount;
-    uint32_t order[XGM_MAX_TERMS];
-    bool any_absent = false, group_absent = false;
-    for (uint32_t j = 0; j < n; ++j) any_absent |= (ltf[j] == 0);
-    /* bounds of the nested tree around the base: MultiAnd(base, filter) → AndNot(…, OR of excluded) */
-    auto group_bounds = [&](TfNode cur) {
-        if (nfilter) {
-            /* QueryFilter::postlist: MultiAndPostList of [base, Query(OP_AND, boolean terms)] */
-            const uint32_t* ftf = ltf + n;
-            TfNode f{ftf[0], ftf[0], ftf[0]};
-            if (nfilter > 1) {
-                TfIdx fin[XGM_MAX_TERMS], fo[XGM_MAX_TERMS];
-                for (uint32_t j = 0; j < nfilter; ++j) { fin[j].tf = ftf[j]; fin[j].idx = j; }
-                std::partial_sort_copy(fin, fin + nfilter, fo, fo + nfilter, [](const TfIdx& a, const TfIdx& c) { return a.tf < c.tf; });
-                uint32_t fs = fo[0].tf;
-                if (fs) for (uint32_t i = 1; i < nfilter; ++i) {
-                    uint32_t old = fs; fs += fo[i].tf;
-                    if (fs >= old && fs <= ix->doccount) { fs = 0; break; }
-                    fs -= ix->doccount;
-                }
-                f.mn = fs;
-                f.mx = fo[0].tf;
-                for (uint32_t i = 1; i < nfilter; ++i) f.mx = std::min(f.mx, fo[i].tf);
-                double fr = fo[0].tf;
-                for (uint32_t i = 1; i < nfilter; ++i) fr = (fr * fo[i].tf) / dbsize;
-                f.est = ix->doccount ? (uint32_t)(fr + 0.5) : 0;
-            }
-            TfNode c0 = cur, c1 = f; /* children in ascending-estimate order */
-            if (f.est < cur.est) { c0 = f; c1 = cur; }
-            uint32_t ms = c0.mn;
-            if (ms) {
-                uint32_t old = ms; ms += c1.mn;
-                if (ms >= old && ms <= ix->doccount) ms = 0; else ms -= ix->doccount;
-            }
-            cur.mn = ms;
-            cur.mx = std::min(c0.mx, c1.mx);
-            cur.est = ix->doccount ? (uint32_t)(((double)c0.est * (double)c1.est) / dbsize + 0.5) : 0;
-        }
-        if (nnot) {
-            /* AndNotPostList::get_termfreq_min/max/est, matcher/andnotpostlist.cc:30-62 */
-            const TfNode rr = or_group_node(ltf + n + nfilter, nnot, ix->doccount);
-            const TfNode a = cur;
-            cur.mn = a.mn <= rr.mx ? 0 : a.mn - rr.mx;
-            cur.mx = std::min(ix->doccount - rr.mn, a.mx);
-            if (ix->doccount == 0) cur.est = 0;
-            else {
-                double e = a.est;
-                e = (e * (double)(ix->doccount - rr.est)) / dbsize;
-                cur.est = (uint32_t)(e + 0.5);
-            }
-        }
-        return cur;
-    };
-    if (q.op == XGM_OP_AND || n == 1) {
-        /* children of the MultiAndPostList: the base terms and, for a Xapiand range, its source — sorted by
-         * get_termfreq_est with the very call of multiandpostlist.h:126-131 */
-        const uint32_t nch = n + (mv_source ? 1u : 0u);
-        const uint32_t src_vf = mv_source ? ix->slot_freq[q.filter_slot] : 0u;
-        TfIdx in[XGM_MAX_TERMS + 1], outv[XGM_MAX_TERMS + 1];
-        for (uint32_t j = 0; j < n; ++j) { in[j].tf = ltf[j]; in[j].idx = j; }
-        if (mv_source) { in[n].tf = src_vf; in[n].idx = n; }
-        std::partial_sort_copy(in, in + nch, outv, outv + nch, [](const TfIdx& a, const TfIdx& c) { return a.tf < c.tf; });
-        uint32_t src_pos = XGM_NO_SRC;
-        {
-            uint32_t k = 0;
-            for (uint32_t j = 0; j < nch; ++j) {
-                if (outv[j].idx == n && mv_source) src_pos = k;
-                else order[k++] = outv[j].idx;
-            }
-        }
-        /* MultiAndPostList::recalc_maxweight / get_termfreq_{min,max,est}, multiandpostlist.cc:55-105,161-171,
-         * over the children in that order (child = base term order[i], or the source at src_pos) */
-        auto ch_min = [&](uint32_t c) { return outv[c].idx == n && mv_source ? 0u : ltf[outv[c].idx]; };
-        auto ch_max = [&](uint32_t c) { return outv[c].idx == n && mv_source ? src_vf : ltf[outv[c].idx]; };
-        double mp = 0, mp_real = 0;
-        for (uint32_t c = 0; c < nch; ++c) {
-            if (outv[c].idx == n && mv_source) { mp += src_weighted ? src_w * 1.7976931348623157e308 : 0.0; mp_real += src_w; }
-            else { mp += maxpart[outv[c].idx]; mp_real += maxpart[outv[c].idx]; }
-        }
-        pq.max_possible = nch == 1 ? maxpart[0] : mp;
-        pq.bucket_max = nch == 1 ? maxpart[0] : mp_real;
-        uint32_t sum = ch_min(0);
-        if (sum) {
-            for (uint32_t i = 1; i < nch; ++i) {
-                uint32_t old = sum;
-                sum += ch_min(i);
-                if (sum >= old && sum <= ix->doccount) { sum = 0; break; }
-                sum -= ix->doccount;
-            }
-        }
-        pq.tf_min = sum;
-        pq.tf_max = ch_max(0);
-        for (uint32_t i = 1; i < nch; ++i) pq.tf_max = std::min(pq.tf_max, ch_max(i));
-        double r = ch_max(0);
-        for (uint32_t i = 1; i < nch; ++i) r = (r * ch_max(i)) / dbsize;
-        pq.tf_est = ix->doccount ? (uint32_t)(r + 0.5) : 0;
-        if (src_weighted) { dq.src_pos = src_pos; dq.src_weight = src_w; }
-        pq.mv_source = mv_source;
-        dq.route = XGM_ROUTE_AND;
-        auto put_term = [&](uint32_t slot, uint32_t j, bool weighted) {
-            dq.terms[slot].termweight = weighted ? tw[j] : 0.0; /* a boolean leaf contributes +0.0: sums unchanged */
-            dq.terms[slot].maxpart = weighted ? maxpart[j] : 0.0;
-            dq.terms[slot].bm_off = XGM_NO_BITMAP; dq.terms[slot].rk_off = 0;
-            dq.terms[slot].blk_begin = 0; dq.terms[slot].nblocks = 0;
-            if (ids[j] != 0xffffffffu) {
-                const TermInfo& tinf = ix->terms[ids[j]];
-                dq.terms[slot].blk_begin = tinf.blk_begin; dq.terms[slot].nblocks = tinf.nblocks;
-                dq.terms[slot].bm_off = tinf.bm_off; dq.terms[slot].rk_off = tinf.rk_off;
-            }
-        };
-        if (ngroups == 0) {
-            for (uint32_t i = 0; i < n; ++i) put_term(i, order[i], true);
-        } else {
-            const TfNode cur = group_bounds(TfNode{pq.tf_min, pq.tf_max, pq.tf_est});
-            pq.tf_min = cur.mn; pq.tf_max = cur.mx; pq.tf_est = cur.est;
-            /* device lists: required = base (its own MultiAndPostList order, which fixes the order of the
-             * weight sum) merged with the boolean filter terms by ascending termfreq; then the excluded lists
-             * that exist in this index */
-            TfIdx fin[XGM_MAX_TERMS], fo[XGM_MAX_TERMS];
-            for (uint32_t j = 0; j < nfilter; ++j) { fin[j].tf = ltf[n + j]; fin[j].idx = n + j; any_absent |= (ltf[n + j] == 0); }
-            std::stable_sort(fin, fin + nfilter, [](const TfIdx& a, const TfIdx& c) { return a.tf < c.tf; });
-            (void)fo;
-            uint32_t slot = 0, bi = 0, fi = 0;
-            while (bi < n || fi < nfilter) {
-                if (fi >= nfilter || (bi < n && ltf[order[bi]] <= fin[fi].tf)) put_term(slot++, order[bi++], true);
-                else put_term(slot++, fin[fi++].idx, false);
-            }
-            uint32_t kept = 0;
-            for (uint32_t j = 0; j < nnot; ++j) {
-                const uint32_t t = n + nfilter + j;
-                if (ltf[t] == 0) continue; /* nothing to exclude */
-                put_term(slot++, t, false);
-                ++kept;
-            }
-            dq.nnot = kept;
-            if (nmaybe) {
-                /* AndMaybePostList: termfreqs are the left's; recalc_maxweight = pl_max + r_max where r is the
-                 * OrContext tree over the optional leaves (matcher/andmaybepostlist.cc:69-75) */
-                const uint32_t mb = n + nfilter + nnot;
-                double mtw[XGM_MAX_TERMS], mmax[XGM_MAX_TERMS];
-                for (uint32_t j = 0; j < nmaybe; ++j) {
-                    const uint32_t gtf = q.stats ? q.stats->termfreq[mb + j] : ltf[mb + j];
-                    mtw[j] = bm25_termweight(N, gtf, q.wqf ? q.wqf[mb + j] : 1, 1.0, k1, k3);
-                    const uint32_t wub = ids[mb + j] == 0xffffffffu ? 0 : ix->terms[ids[mb + j]].wdf_ub;
-                    mmax[j] = bm25_maxpart(mtw[j], len_factor, k1, b, mnl, wub, ix->doclen_lb);
-                }
-                double rmax = mmax[0];
-                dq.prog_len = 0;
-                if (nmaybe == 1) {
-                    dq.prog[dq.prog_len++] = 0;
-                } else {
-                    OrTree tr;
-                    build_or_tree(ltf + mb, nmaybe, tr);
-                    int stack[4 * XGM_MAX_TERMS], sp = 0, outrev[2 * XGM_MAX_TERMS], nr = 0;
-                    stack[sp++] = tr.root;
-                    while (sp) {
-                        int x = stack[--sp];
-                        outrev[nr++] = x;
-                        if (x >= (int)nmaybe) { stack[sp++] = tr.lch[x]; stack[sp++] = tr.rch[x]; }
-                    }
-                    double sm[2 * XGM_MAX_TERMS];
-                    int pp = 0;
-                    for (int i = nr - 1; i >= 0; --i) {
-                        int x = outrev[i];
-                        if (x < (int)nmaybe) { dq.prog[dq.prog_len++] = (int8_t)x; sm[pp++] = mmax[x]; }
-                        else { dq.prog[dq.prog_len++] = -1; --pp; sm[pp - 1] = sm[pp - 1] + sm[pp]; }
-                    }
-                    rmax = sm[0];
-                }
-                pq.max_possible = pq.max_possible + rmax;
-                pq.bucket_max = pq.max_possible;
-                for (uint32_t j = 0; j < nmaybe; ++j) {
-                    put_term(slot, mb + j, false);
-                    dq.terms[slot].termweight = mtw[j];
-                    dq.terms[slot].maxpart = mmax[j];
-                    ++slot;
-                }
-                dq.nmaybe = nmaybe;
-                pq.aux_subqs = true;
-                pq.nterms = nweighted_base + nmaybe; /* total weighted leaves, for the percentage scale */
-            }
-        }
-    } else {
-        /* OR of leaves: Huffman-shaped tree of binary OrPostLists, built from the leaves in query order
-         * (OrContext::postlist, queryinternal.cc:440-489). On the device the leaves are stored in
-         * ascending-termfreq order (position = ownership priority); the program refers to positions. */
-        OrTree tr;
-        build_or_tree(ltf, n, tr);
-        TfIdx in[XGM_MAX_TERMS];
-        for (uint32_t j = 0; j < n; ++j) { in[j].tf = ltf[j]; in[j].idx = j; }
-        std::stable_sort(in, in + n, [](const TfIdx& a, const TfIdx& c) { return a.tf < c.tf; });
-        uint32_t posof[XGM_MAX_TERMS];
-        for (uint32_t i = 0; i < n; ++i) { order[i] = in[i].idx; posof[in[i].idx] = i; }
-        int stack[4 * XGM_MAX_TERMS], sp = 0, outrev[2 * XGM_MAX_TERMS], nr = 0;
-        stack[sp++] = tr.root;
-        while (sp) {
-            int x = stack[--sp];
-            outrev[nr++] = x;
-            if (x >= (int)n) { stack[sp++] = tr.lch[x]; stack[sp++] = tr.rch[x]; }
-        }
-        double sm[2 * XGM_MAX_TERMS], se[2 * XGM_MAX_TERMS];
-        uint32_t smin[2 * XGM_MAX_TERMS], smax[2 * XGM_MAX_TERMS];
-        int p = 0;
-        dq.prog_len = 0;
-        for (int i = nr - 1; i >= 0; --i) {
-            int x = outrev[i];
-            if (x < (int)n) {
-                dq.prog[dq.prog_len++] = (int8_t)posof[x];
-                sm[p] = maxpart[x]; se[p] = smin[p] = smax[p] = ltf[x]; ++p;
-            } else {
-                dq.prog[dq.prog_len++] = -1;
-                --p;
-                sm[p - 1] = sm[p - 1] + sm[p];
-                smin[p - 1] = std::max(smin[p - 1], smin[p]);
-                uint32_t lm = smax[p - 1], t = lm + smax[p];
-                if (t > ix->doccount || t < lm) t = ix->doccount;
-                smax[p - 1] = t;
-                double a = (double)(uint32_t)se[p - 1], c2 = (double)(uint32_t)se[p];
-                se[p - 1] = dbsize == 0.0 ? 0 : (uint32_t)(a + c2 - (a * c2 / dbsize) + 0.5);
-            }
-        }
-        pq.max_possible = sm[0]; pq.tf_min = smin[0]; pq.tf_max = smax[0]; pq.tf_est = (uint32_t)se[0];
-        pq.bucket_max = pq.max_possible;
-        dq.route = XGM_ROUTE_OR;
-        auto put_leaf = [&](uint32_t slot, uint32_t j, bool weighted) {
-            dq.terms[slot].termweight = weighted ? tw[j] : 0.0;
-            dq.terms[slot].maxpart = weighted ? maxpart[j] : 0.0;
-            dq.terms[slot].bm_off = XGM_NO_BITMAP; dq.terms[slot].rk_off = 0;
-            dq.terms[slot].blk_begin = 0; dq.terms[slot].nblocks = 0;
-            if (ids[j] != 0xffffffffu) {
-                const TermInfo& tinf = ix->terms[ids[j]];
-                dq.terms[slot].blk_begin = tinf.blk_begin; dq.terms[slot].nblocks = tinf.nblocks;
-                dq.terms[slot].bm_off = tinf.bm_off; dq.terms[slot].rk_off = tinf.rk_off;
-            }
-        };
-        for (uint32_t i = 0; i < n; ++i) put_leaf(i, order[i], true);
-        if (ngroups) {
-            /* QueryFilter / QueryAndNot above the OrPostList tree: the filter's boolean terms and the excluded
-             * terms weigh nothing (MultiAndPostList::get_weight adds +0.0, AndNotPostList returns the left's
-             * weight), so a match keeps the tree's weight; the counts follow the same bound arithmetic as around
-             * an AND base.  The device keeps them behind the leaves: terms[n .. n + or_nreq) must hold the
-             * document, terms[n + or_nreq .. + nnot) must not. */
-            const TfNode cur = group_bounds(TfNode{pq.tf_min, pq.tf_max, pq.tf_est});
-            pq.tf_min = cur.mn; pq.tf_max = cur.mx; pq.tf_est = cur.est;
-            dq.nterms = n;
-            uint32_t slot = n;
-            for (uint32_t j = 0; j < nfilter; ++j) { put_leaf(slot++, n + j, false); group_absent |= (ltf[n + j] == 0); }
-            dq.or_nreq = nfilter;
-            uint32_t kept = 0;
-            for (uint32_t j = 0; j < nnot; ++j) {
-                if (ltf[n + nfilter + j] == 0) continue; /* nothing to exclude */
-                put_leaf(slot++, n + nfilter + j, false);
-                ++kept;
-            }
-            dq.nnot = kept;
-        }
-    }
+    if (q.op == XGM_OP_AND || t.n == 1) plan_and_route(ix, q, t, pq, dq);
+    else plan_or_route(ix, t, pq, dq);
+
     /* algorithmic bytes, SURVEY.md §8(d): compressed columns + 16 B per block header of every query
      * term (full lists, no credit for skipping) + 16 B per result; 4 B per candidate added at wait() */
-    for (uint32_t j = 0; j < nall; ++j)
-        if (ids[j] != 0xffffffffu) pq.alg_bytes += ix->terms[ids[j]].bytes;
+    for (uint32_t j = 0; j < t.n + t.ngroups; ++j)
+        if (t.ids[j] != 0xffffffffu) pq.alg_bytes += ix->terms[t.ids[j]].bytes;
     pq.alg_bytes += 16ull * pq.topk;
 
     /* `first` at or beyond the largest possible match count: ProtoMSet never fills (protomset.h:497-505),
      * the MSet is empty and all three bounds equal the exact match count — count on the device only */
     if (pq.first >= pq.tf_max && cal != 0) { pq.count_only = true; dq.topk = 0; }
-    else if (pq.topk > s->max_topk) { pq.status = XGM_E_INVALID; return XGM_OK; }
+    else if (pq.topk > s->max_topk) { pq.status = XGM_E_INVALID; return; }
     /* pruning buckets: linear in the primary sort key (weight, or the sort value for VAL sorts) */
     if (q.sort_by == XGM_SORT_REL || q.sort_by == XGM_SORT_REL_VAL) {
         dq.bucket_scale = pq.bucket_max > 0 ? (double)XGM_NBINS / pq.bucket_max : 0.0;
@@ -1674,11 +1647,12 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
 
     /* percent_scale_factor needs the number of subqueries matching the best-WEIGHTED document: when that varies
      * per document and the order is not by weight alone, have the kernels log the running-maximum matches */
-    dq.log_raises = ((dq.route == XGM_ROUTE_OR && n > 1) || pq.aux_subqs) && q.sort_by != XGM_SORT_REL ? 1u : 0u;
+    dq.log_raises = (dq.route == XGM_ROUTE_OR || pq.aux_subqs) && q.sort_by != XGM_SORT_REL ? 1u : 0u;
     pq.log_raises = dq.log_raises != 0;
-    if (cal == 0) { pq.on_device = false; return XGM_OK; } /* bounds only, matcher.cc:437-461 */
-    if (dq.route == XGM_ROUTE_AND && any_absent) { pq.on_device = false; return XGM_OK; } /* AND with an absent term: empty */
-    if (dq.route == XGM_ROUTE_OR && group_absent) { pq.on_device = false; return XGM_OK; } /* OR filtered by an absent term: empty */
+    if (cal == 0) return; /* bounds only, matcher.cc:437-461 */
+    /* a list every match is in is absent (an AND's terms, the FILTER terms on either base): the MSet is empty */
+    for (uint32_t j = dq.route == XGM_ROUTE_AND ? 0 : t.n; j < t.n + t.nfilter; ++j)
+        if (t.ltf[j] == 0) return;
     pq.on_device = true;
     /* one segment per (query[, leaf]); the device expands segments into work items (xgm_expand_items_kernel) */
     if (dq.route == XGM_ROUTE_AND) {
@@ -1686,22 +1660,16 @@ static xgm_status plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, P
         bool all_bm = dq.nterms >= 2;
         for (uint32_t i = 1; i < dq.nterms + dq.nnot; ++i) all_bm = all_bm && dq.terms[i].bm_off != XGM_NO_BITMAP;
         std::vector<XgmWorkItem>& dst = all_bm ? segs.bm_list : segs.and_list;
-        XgmWorkItem wi;
-        wi.query = qi; wi.b0 = dq.terms[0].nblocks; wi.b1 = 0; wi.pad = 0;
-        if (wi.b0) dst.push_back(wi);
+        if (dq.terms[0].nblocks) dst.push_back(XgmWorkItem{qi, dq.terms[0].nblocks, 0, 0});
     } else {
-        bool fastor = n <= 5 && ngroups == 0 && !(getenv("XGM_OR_KERNEL") && atoi(getenv("XGM_OR_KERNEL")) == 1);
-        for (uint32_t leaf = 0; leaf < n; ++leaf) fastor = fastor && dq.terms[leaf].bm_off != XGM_NO_BITMAP;
+        bool fastor = t.n <= 5 && t.ngroups == 0 && !s->or_general;
+        for (uint32_t leaf = 0; leaf < t.n; ++leaf) fastor = fastor && dq.terms[leaf].bm_off != XGM_NO_BITMAP;
         /* relevance order, no predicate, results wanted: multi-leaf documents by bitmap union first */
         const bool tile = s->or_tile && q.filter == XGM_FILTER_NONE && q.sort_by == XGM_SORT_REL && dq.topk != 0;
         dq.or_fast = !fastor ? XGM_OR_FAST_GENERAL : tile ? XGM_OR_FAST_TILE : XGM_OR_FAST_OR3;
-        for (uint32_t leaf = 0; leaf < n; ++leaf) {
-            XgmWorkItem wi;
-            wi.query = qi; wi.b0 = dq.terms[leaf].nblocks; wi.b1 = 0; wi.pad = leaf;
-            if (wi.b0) segs.or_list.push_back(wi);
-        }
+        for (uint32_t leaf = 0; leaf < t.n; ++leaf)
+            if (dq.terms[leaf].nblocks) segs.or_list.push_back(XgmWorkItem{qi, dq.terms[leaf].nblocks, 0, leaf});
     }
-    return XGM_OK;
 }
 
 /* Level starts of segments sorted by descending length: level k holds the k-th item of every segment that has one,
@@ -1849,6 +1817,21 @@ static cudaError_t expand_driver_runs(const BmList& L, const XgmBlockHdr* hdr, u
                                     L.d_rng + 2 * n, L.d_rng_total, L.d_exp, cs);
 }
 
+/* The match kernels of one pass (p.pass) over the batch's work lists */
+static xgm_status launch_match(xgm_searcher* s, const XgmKernelParams& p, cudaStream_t cs) {
+    uint32_t& launches = s->stats.kernel_launches;
+    if (s->bm_list.nitems) { CUDA_TRY(xgm_launch_and_bm(p, s->grid_bm, cs)); ++launches; }
+    if (s->and_list.nitems) { CUDA_TRY(xgm_launch_and(p, s->grid, cs)); ++launches; }
+    if (s->or_list.nitems && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p, s->grid_or3, 0, cs)); ++launches; }
+    if (s->or_list.nitems && s->any_or_slow) { CUDA_TRY(xgm_launch_or(p, s->grid_or, cs)); ++launches; }
+    if (s->ntileq) { /* documents with >= 2 leaves by bitmap union, then the single-leaf ones against the threshold */
+        CUDA_TRY(xgm_launch_or_tile(p, s->grid_tile, cs));
+        CUDA_TRY(xgm_launch_or3(p, s->grid_or3, 1, cs));
+        launches += 2;
+    }
+    return XGM_OK;
+}
+
 static xgm_status launch_batch(xgm_searcher* s) {
     XgmKernelParams& p = s->params;
     /* batches that fill the GPU on their own run their kernels on the index's FIFO compute stream; small
@@ -1871,30 +1854,16 @@ static xgm_status launch_batch(xgm_searcher* s) {
     CUDA_TRY(s->bm_list.range_mode ? expand_driver_runs(s->bm_list, p.hdr, s->range_bits, s->bpi, cs, launches)
                                    : expand_levels(s->bm_list, s->bpi, cs, launches));
     CUDA_TRY(cudaEventRecord(s->ev0, cs));
-    if (s->bm_list.nitems) { CUDA_TRY(xgm_launch_and_bm(p, s->grid_bm, cs)); s->stats.kernel_launches++; }
-    if (s->and_list.nitems) { CUDA_TRY(xgm_launch_and(p, s->grid, cs)); s->stats.kernel_launches++; }
-    if (s->or_list.nitems && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p, s->grid_or3, 0, cs)); s->stats.kernel_launches++; }
-    if (s->or_list.nitems && s->any_or_slow) { CUDA_TRY(xgm_launch_or(p, s->grid_or, cs)); s->stats.kernel_launches++; }
-    if (s->ntileq) { /* documents with >= 2 leaves by bitmap union, then the single-leaf ones against the threshold */
-        CUDA_TRY(xgm_launch_or_tile(p, s->grid_tile, cs));
-        CUDA_TRY(xgm_launch_or3(p, s->grid_or3, 1, cs));
-        s->stats.kernel_launches += 2;
-    }
+    xgm_status st = launch_match(s, p, cs);
+    if (st != XGM_OK) return st;
     CUDA_TRY(cudaEventRecord(s->ev1, cs));
     CUDA_TRY(xgm_launch_topk(p, s->nq, cs));
     s->stats.kernel_launches += (s->nq >= 64 && p.topk_list) ? 2 : 1; /* xgm_topk_small_kernel + xgm_topk_kernel */
     /* second pass: only queries whose candidate buffer overflowed do any work (device-side flag) */
     XgmKernelParams p2 = p;
     p2.pass = 1;
-    if (s->bm_list.nitems) { CUDA_TRY(xgm_launch_and_bm(p2, s->grid_bm, cs)); s->stats.kernel_launches++; }
-    if (s->and_list.nitems) { CUDA_TRY(xgm_launch_and(p2, s->grid, cs)); s->stats.kernel_launches++; }
-    if (s->or_list.nitems && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p2, s->grid_or3, 0, cs)); s->stats.kernel_launches++; }
-    if (s->or_list.nitems && s->any_or_slow) { CUDA_TRY(xgm_launch_or(p2, s->grid_or, cs)); s->stats.kernel_launches++; }
-    if (s->ntileq) {
-        CUDA_TRY(xgm_launch_or_tile(p2, s->grid_tile, cs));
-        CUDA_TRY(xgm_launch_or3(p2, s->grid_or3, 1, cs));
-        s->stats.kernel_launches += 2;
-    }
+    st = launch_match(s, p2, cs);
+    if (st != XGM_OK) return st;
     CUDA_TRY(xgm_launch_topk(p2, s->nq, cs));
     s->stats.kernel_launches++;
     CUDA_TRY(cudaEventRecord(s->ev2, cs));
@@ -1924,23 +1893,15 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     int T = 1;
     if (nq >= 512) T = PlannerPool::get().threads();
     if (T <= 1) {
-        for (uint32_t i = 0; i < nq; ++i) {
-            xgm_status st = plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], segs);
-            if (st != XGM_OK) return st;
-        }
+        for (uint32_t i = 0; i < nq; ++i) plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], segs);
     } else {
         std::vector<PlannedSegments> ts(T);
-        std::vector<xgm_status> tst(T, XGM_OK);
         PlannerPool::get().run(T, [&](int t) {
             uint32_t a = (uint32_t)((uint64_t)nq * t / T), b = (uint32_t)((uint64_t)nq * (t + 1) / T);
             ts[t].bm_list.reserve((size_t)(b - a));
-            for (uint32_t i = a; i < b; ++i) {
-                xgm_status st = plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], ts[t]);
-                if (st != XGM_OK) { tst[t] = st; return; }
-            }
+            for (uint32_t i = a; i < b; ++i) plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], ts[t]);
         });
         for (int t = 0; t < T; ++t) {
-            if (tst[t] != XGM_OK) return fail(tst[t], "query planning failed");
             segs.and_list.insert(segs.and_list.end(), ts[t].and_list.begin(), ts[t].and_list.end());
             segs.or_list.insert(segs.or_list.end(), ts[t].or_list.begin(), ts[t].or_list.end());
             segs.bm_list.insert(segs.bm_list.end(), ts[t].bm_list.begin(), ts[t].bm_list.end());
@@ -2029,7 +1990,7 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     return XGM_OK;
 }
 
-static void finish_info(const PlannedQuery& pq, const XgmDevResult* dr, const double* w, const uint64_t* keys, bool is_or,
+static void finish_info(const PlannedQuery& pq, const XgmDevResult* dr, const uint64_t* keys, bool is_or,
                         xgm_mset_info* o, const XgmRaise* raises = nullptr, uint32_t nraise = 0) {
     memset(o, 0, sizeof(*o));
     o->first = pq.first;
@@ -2042,7 +2003,6 @@ static void finish_info(const PlannedQuery& pq, const XgmDevResult* dr, const do
     if (pq.on_device) {
         size = dr->n; known = dr->known; o->exact_matches = dr->exact;
         max_w = dr->max_w;
-        (void)w;
         /* ProtoMSet::finalise, protomset.h:484-612 (no collapser / decider / percent cut-off) */
         if (pq.count_only) { size = 0; lb = est = ub = dr->exact; }
         else if (size != pq.topk) lb = est = ub = size;
@@ -2088,7 +2048,7 @@ static void finish_info(const PlannedQuery& pq, const XgmDevResult* dr, const do
          * ExternalPostList::count_matching_subqs return 1) without being one of the total weighted leaves
          * (api/queryinternal.cc:1097-1098) */
         if (pq.filter) subqs += 1;
-        double percent_scale = (double)subqs / (double)pq.nterms;
+        double percent_scale = (double)subqs / (double)pq.nweighted;
         percent_scale /= max_w;
         o->percent_scale_factor = percent_scale * 100.0;
     }
@@ -2197,7 +2157,7 @@ extern "C" xgm_status xgm_search_wait(xgm_searcher* s, uint32_t* docids, double*
         const PlannedQuery& pq = s->plan[i];
         const size_t off = (size_t)i * s->max_topk;
         if (pq.status == XGM_OK && pq.on_device && (s->h_info[i].flags & XGM_RES_SECOND_PASS)) s->stats.second_pass_queries++;
-        finish_info(pq, &s->h_info[i], s->h_out_w + off, s->any_sort ? s->h_out_k + off : nullptr,
+        finish_info(pq, &s->h_info[i], s->any_sort ? s->h_out_k + off : nullptr,
                     s->h_queries[i].route == XGM_ROUTE_OR || pq.aux_subqs, &info[i],
                     s->any_raise ? s->h_raise + (size_t)i * XGM_RAISE_LOG : nullptr, s->any_raise ? s->h_qstate[i].nraise : 0u);
         if (pq.status == XGM_OK && pq.on_device) s->stats.algorithmic_bytes += 4ull * s->h_info[i].exact;
