@@ -121,7 +121,7 @@ typedef struct xgm_index_info {
     uint64_t bytes_docids, bytes_wdfs, bytes_headers, bytes_doclen; /* HBM footprint by column */
     int device;
     uint64_t revision;
-    uint64_t bytes_bitmaps;  /* membership bitmaps + rank directories of the frequent terms */
+    uint64_t bytes_bitmaps;  /* membership bitmaps, their coarse bitmaps (a bit per 8 docids) + rank directories of the frequent terms */
     uint32_t nbitmaps;
 } xgm_index_info;
 xgm_status xgm_index_info_get(const xgm_index*, xgm_index_info* out);

@@ -1,6 +1,6 @@
 """Work of the bitmap AND list for bench.py's C2 and C5 batches (step 0): driver blocks the AND kernel decodes when
 every query decodes its own driver (one item list per query) and when the queries that share a driver share the
-decode (runs of up to 3 queries), computed from the index's term frequencies; and the work items of the list as
+decode (runs of up to RUN queries), computed from the index's term frequencies; and the work items of the list as
 the library in this tree plans them (one batch on the GPU).  Prints one JSON line per configuration."""
 import collections
 import json
@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench  # noqa: E402
 from xapiand_b200 import xgm  # noqa: E402
 
-RUN = 3  # XGM_BM_RUN
+RUN = 6  # XGM_BM_RUN
 BLOCK = 128  # postings per block
 
 

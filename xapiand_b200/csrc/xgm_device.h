@@ -49,6 +49,7 @@ struct XgmKernelParams {
     const uint4* tfs;
     const uint32_t* doclen;
     const uint32_t* bitmaps;
+    const uint32_t* coarse;       /* a bit per 8 docids of bitmaps[]: word bm_off / 8 + (d >> 8), bit (d >> 3) & 31 */
     const uint32_t* ranks;
     uint32_t lastdocid;
     uint32_t doclen_lb;           /* Database::get_doclength_lower_bound: block-level weight bounds */
@@ -114,6 +115,7 @@ cudaError_t xgm_launch_or_tile(const XgmKernelParams& p, int grid, cudaStream_t 
 int xgm_or_tile_occupancy_blocks_per_sm();
 int xgm_or3_occupancy_blocks_per_sm();
 cudaError_t xgm_launch_topk(const XgmKernelParams& p, uint32_t nq, cudaStream_t s);
+cudaError_t xgm_launch_coarse(const uint32_t* bitmaps, size_t ncoarse, uint32_t* coarse, cudaStream_t s);
 cudaError_t xgm_launch_decode(const XgmKernelParams& p, uint32_t blk_begin, uint32_t nblocks, uint32_t* out_d,
                               uint32_t* out_w, cudaStream_t s);
 size_t xgm_topk_smem_bytes(uint32_t keep_cap);

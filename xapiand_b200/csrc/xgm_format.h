@@ -16,6 +16,9 @@
  *           bitmap costs at most XGM_BITMAP_K bits per posting.  HBM is plentiful (80 GB) and the
  *           leapfrog of an AND is at heart a membership test: probing a bitmap replaces decoding the
  *           longer lists entirely; the rank directory gives the posting's index, hence its wdf.
+ *   coarse[] next to every bitmap, one bit per 8 docids (built on the device at upload): coarse word
+ *           bm_off / 8 + (d >> 8) covers the 256-docid group of docid d, bit (d >> 3) & 31 is set if any
+ *           of its 8 docids is in the list.  A bitmap is 8 words per group, so bm_off is a multiple of 8.
  *   doclen[] dense u32 per docid (the reference keeps a second vbyte stream under key "\0\xe0",
  *           glass_postlist.cc:194-205,994-1021).
  */
@@ -84,6 +87,7 @@ struct XgmDevQuery {
     uint32_t or_fast;                   /* OR: the kernels that produce its union, XGM_OR_FAST_* */
     uint32_t or_nreq;                   /* OR under OP_FILTER: terms[nterms .. nterms+or_nreq) must hold the document, then nnot excluded ones */
     uint32_t log_raises;                /* record the matches that attain the running maximum weight (XGM_RAISE_LOG) */
+    uint32_t probe_coarse;              /* bitmap AND: test terms[1]'s coarse bit before its fine bit (sparse terms[1]) */
     XgmDevTerm terms[XGM_DEV_MAX_TERMS]; /* AND: ascending termfreq (MultiAndPostList order) */
 };
 
@@ -97,7 +101,7 @@ struct XgmWorkItem {
  * which decodes the driver's blocks once for all of them.  Longer runs decode less but make fewer, longer items per
  * docid range, so more ranges are in flight at once and their bitmap slices outgrow L2 (DESIGN.md §6).  The AND
  * kernel tags a queued candidate with its query's slot in the run in 4 bits: at most 16. */
-#define XGM_BM_RUN 3
+#define XGM_BM_RUN 6
 
 /* per-query running state of a batch (zeroed before every launch) */
 struct XgmQState {

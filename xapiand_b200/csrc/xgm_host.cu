@@ -128,6 +128,7 @@ struct xgm_index {
     uint4* d_tfs = nullptr;
     uint32_t* d_doclen = nullptr;
     uint32_t* d_bitmaps = nullptr;
+    uint32_t* d_coarse = nullptr; /* a bit per 8 docids of d_bitmaps (xgm_format.h) */
     uint32_t* d_ranks = nullptr;
     uint32_t* d_voff[XGM_MAX_SLOTS] = {};
     uint64_t* d_vals[XGM_MAX_SLOTS] = {};
@@ -298,7 +299,15 @@ static xgm_status upload_index(xgm_index* ix, std::vector<Chunk>& chunks, const 
         std::vector<uint32_t>().swap(chunks[i].bitmaps);
         std::vector<uint32_t>().swap(chunks[i].ranks);
     }
-    ix->bytes_bitmaps = (nbm + nrk) * 4;
+    /* the coarse bitmaps: one word per 8 fine words, so a term's coarse word of docid d is coarse[bm_off / 8 + (d >> 8)] */
+    for (const auto& t : ix->terms)
+        if (t.bm_off != XGM_NO_BITMAP && (t.bm_off & 7u) != 0)
+            return fail(XGM_E_INVALID, "membership bitmap offset %llu is not a multiple of 8 words", (unsigned long long)t.bm_off);
+    const size_t ncoarse = nbm / 8;
+    CUDA_TRY(cudaMalloc(&ix->d_coarse, std::max<size_t>(ncoarse, 8) * 4));
+    CUDA_TRY(xgm_launch_coarse(ix->d_bitmaps, ncoarse, ix->d_coarse, 0));
+    CUDA_TRY(cudaDeviceSynchronize());
+    ix->bytes_bitmaps = (nbm + ncoarse + nrk) * 4;
     /* +16 bytes slack at the end of each column: the unpackers may read one word past a block */
     CUDA_TRY(cudaMalloc(&ix->d_hdr, (nh + 1) * sizeof(XgmBlockHdr)));
     CUDA_TRY(cudaMalloc(&ix->d_docs, nd * 4 + 64));
@@ -535,7 +544,7 @@ extern "C" void xgm_index_close(xgm_index* ix) {
     if (!ix) return;
     cudaSetDevice(ix->device);
     cudaFree(ix->d_hdr); cudaFree(ix->d_docs); cudaFree(ix->d_tfs); cudaFree(ix->d_doclen);
-    cudaFree(ix->d_bitmaps); cudaFree(ix->d_ranks);
+    cudaFree(ix->d_bitmaps); cudaFree(ix->d_coarse); cudaFree(ix->d_ranks);
     for (int s = 0; s < XGM_MAX_SLOTS; ++s) { cudaFree(ix->d_voff[s]); cudaFree(ix->d_vals[s]); }
     if (ix->compute_stream) cudaStreamDestroy(ix->compute_stream);
     delete ix;
@@ -801,7 +810,7 @@ extern "C" xgm_status xgm_term_stats_many(const xgm_index* ix, uint32_t n, const
 static void fill_index_params(const xgm_index* ix, XgmKernelParams& p) {
     memset(&p, 0, sizeof(p));
     p.hdr = ix->d_hdr; p.docs = ix->d_docs; p.tfs = ix->d_tfs; p.doclen = ix->d_doclen; p.lastdocid = ix->lastdocid;
-    p.bitmaps = ix->d_bitmaps; p.ranks = ix->d_ranks; p.doclen_lb = ix->doclen_lb;
+    p.bitmaps = ix->d_bitmaps; p.coarse = ix->d_coarse; p.ranks = ix->d_ranks; p.doclen_lb = ix->doclen_lb;
     for (int s = 0; s < XGM_MAX_SLOTS; ++s) { p.slots[s].voff = ix->d_voff[s]; p.slots[s].vals = ix->d_vals[s]; }
 }
 
@@ -1027,7 +1036,7 @@ struct xgm_searcher {
     OrList or_list;
     BmList bm_list;    /* bitmap AND kernel */
     uint32_t bpi = 16;
-    uint32_t range_bits = 17; /* XGM_RANGE_BITS: 2^17 docids per range (DESIGN.md §3.1) */
+    uint32_t range_bits = 16; /* XGM_RANGE_BITS: 2^16 docids per range (DESIGN.md §3.1) */
     uint32_t* d_topk_list = nullptr; /* [max_batch] queries left to the CTA-per-query top-k kernel */
     unsigned char* d_ctrl = nullptr; /* [XGM_CTRL_HDR B work counters][nq x XgmQState][nq x XGM_NBINS x u32] */
     double* d_match_w = nullptr;
@@ -1490,6 +1499,10 @@ static TfNode group_bounds(const xgm_index* ix, const PlanTerms& t, TfNode cur) 
     return cur;
 }
 
+/* Largest expected share of driver postings whose coarse bit in terms[1] is set, 1 - (1 - tf / lastdocid)^8, for
+ * which the bitmap AND kernel tests the coarse bit first (DESIGN.md §6: chosen by measurement on C2 and C5). */
+#define XGM_COARSE_PASS_MAX 0.1
+
 /* An AND base: one MultiAndPostList over the base terms and, for a Xapiand range, its source; the FILTER terms join
  * the required lists as boolean leaves, then the AND_NOT and AND_MAYBE terms follow. */
 static void plan_and_route(const xgm_index* ix, const xgm_query& q, const PlanTerms& t, PlannedQuery& pq,
@@ -1539,14 +1552,18 @@ static void plan_and_route(const xgm_index* ix, const xgm_query& q, const PlanTe
     TfIdx fin[XGM_MAX_TERMS];
     for (uint32_t j = 0; j < t.nfilter; ++j) fin[j] = TfIdx{t.ltf[n + j], n + j};
     std::stable_sort(fin, fin + t.nfilter, tf_less);
-    uint32_t slot = 0, bi = 0, fi = 0;
+    uint32_t slot = 0, bi = 0, fi = 0, tf1 = 0;
     while (bi < n || fi < t.nfilter) {
-        if (fi >= t.nfilter || (bi < n && t.ltf[order[bi]] <= fin[fi].tf)) {
-            const uint32_t j = order[bi++];
-            put_term(ix, dq.terms[slot++], t.ids[j], t.tw[j], t.maxpart[j]);
-        } else {
-            put_term(ix, dq.terms[slot++], t.ids[fin[fi++].idx], 0.0, 0.0);
-        }
+        const bool base = fi >= t.nfilter || (bi < n && t.ltf[order[bi]] <= fin[fi].tf);
+        const uint32_t j = base ? order[bi++] : fin[fi++].idx;
+        if (slot == 1) tf1 = t.ltf[j];
+        put_term(ix, dq.terms[slot++], t.ids[j], base ? t.tw[j] : 0.0, base ? t.maxpart[j] : 0.0);
+    }
+    /* The bitmap AND kernel probes terms[1] for every driver posting.  Where a coarse bit (8 docids) is rarely set,
+     * testing it first leaves few fine-word loads; where it is mostly set, the second load only adds latency. */
+    if (dq.nterms >= 2 && ix->lastdocid != 0) {
+        const double pass = 1.0 - std::pow(1.0 - std::min(1.0, (double)tf1 / ix->lastdocid), 8.0);
+        dq.probe_coarse = pass <= XGM_COARSE_PASS_MAX ? 1u : 0u;
     }
     slot = put_excluded(ix, t, dq, slot);
     if (t.nmaybe) {

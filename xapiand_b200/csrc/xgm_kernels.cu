@@ -11,6 +11,7 @@
  *   xgm_topk_small_kernel   ProtoMSet top-k + match counting (protomset.h:295-400,484-683; msetcmp.cc:54-98):
  *   xgm_topk_kernel         a warp per query with a handful of matches, a CTA per query otherwise
  *   xgm_merge_kernel        merge of the per-shard top-k lists (Matcher::merge_mset)
+ *   xgm_coarse_kernel       the coarse bitmaps (a bit per 8 docids) from the membership bitmaps, at index upload
  *   xgm_decode_kernel       round-trip decode of one term (index self-check)
  *   xgm_expand_items_kernel work items of a level-ordered list from its segments
  *   xgm_range_{count,scan,fill}_kernel   work items of the range-major bitmap AND list
@@ -873,7 +874,8 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, 4) xgm_and_bm3_kernel(const __
     bool done = false;
     /* current work item: its driver blocks are hdr[drv + i], i < it_n; those from db on are left to decode */
     uint32_t drv = 0, it_n = 0, db = 0, cur = 0;
-    /* the item's run: lane s holds the query of slot s and the offset of its probe bitmap (terms[1]).  run_bits: low
+    /* the item's run: lane s holds the query of slot s and the offset of its probe bitmap (terms[1]), or'ed with 1 when
+     * the query probes through the coarse bitmap first (bm_off is a multiple of 8, its low three bits are free).  run_bits: low
      * half, a bit per slot that takes part (in the second pass only the queries that re-run); high half, the slots
      * still to probe on the decoded pair, which sits in buffers cur ^ 2, cur ^ 2 + 1 */
     uint32_t slot_q = 0, run_bits = 0;
@@ -978,7 +980,7 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, 4) xgm_and_bm3_kernel(const __
             const bool take = lane < n && (p.pass == 0 || p.qstate[slot_q].rerun != 0);
             run_bits = __ballot_sync(FULL, take);
             if (run_bits == 0) continue; /* second pass: no query of the run re-runs */
-            slot_bm = take ? p.queries[slot_q].terms[1].bm_off : 0ull;
+            slot_bm = take ? p.queries[slot_q].terms[1].bm_off | p.queries[slot_q].probe_coarse : 0ull;
             drv = p.queries[__shfl_sync(FULL, slot_q, 0)].terms[0].blk_begin + wi.b0;
             it_n = wi.b1 - wi.b0;
             db = 0;
@@ -994,21 +996,38 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, 4) xgm_and_bm3_kernel(const __
         if ((run_bits >> 16) != 0) {
             const uint32_t s = (uint32_t)__ffs(run_bits >> 16) - 1u;
             run_bits ^= 1u << (16 + s);
-            const uint32_t* __restrict__ bm1 = p.bitmaps + __shfl_sync(FULL, slot_bm, s);
+            const uint64_t sbm = __shfl_sync(FULL, slot_bm, s);
+            const uint32_t* __restrict__ bm1 = p.bitmaps + (sbm & ~7ull);
             const uint32_t pb = cur ^ 2u;
             /* slot k of lane l: posting 32 (k & 3) + l of block k >> 2, as the decode step left it */
-            uint32_t c[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) c[k] = ws.dstage[pb + (k >> 2)][32 * (k & 3) + lane];
+#define BM3_POSTING(k) ws.dstage[pb + ((k) >> 2)][32 * ((k) & 3) + lane]
             /* the skip_to/check of the leapfrog: one bitmap word per candidate, all loads issued together */
             uint32_t w[8];
-            /* phases >> 8, bit k: this lane's slot k holds a posting; bit 8: both blocks are full (warp-uniform) */
-            if (phases >> 16) { /* two full blocks: no per-posting predicates */
+            /* phases >> 8, bit k: this lane's slot k holds a posting; bit 8: both blocks are full (warp-uniform).  live,
+             * bit k: slot k is to be tested against the fine bitmap */
+            uint32_t live = (phases >> 8) & 0xffu;
+            if (sbm & 1u) {
+                /* sparse probe list: first the coarse words (a 32-byte sector spans 2048 docids, not 256), then the fine
+                 * word only where the posting's 8-docid group holds a member.  The postings are read from shared memory
+                 * in each phase (the memory clobber keeps them there), so the coarse round trip holds no more registers
+                 * than the fine one: held across it they spill. */
+#pragma unroll
+                for (int k = 0; k < 8; ++k) w[k] = (live >> k & 1u) ? __ldg(p.coarse + (sbm >> 3) + (BM3_POSTING(k) >> 8)) : 0u;
+                live = 0;
+#pragma unroll
+                for (int k = 0; k < 8; ++k) live |= (__funnelshift_r(w[k], 0u, BM3_POSTING(k) >> 3) & 1u) << k;
+                asm volatile("" ::: "memory");
+            }
+            uint32_t c[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) c[k] = BM3_POSTING(k);
+#undef BM3_POSTING
+            if ((phases >> 16) && !(sbm & 1u)) { /* two full blocks: no per-posting predicates */
 #pragma unroll
                 for (int k = 0; k < 8; ++k) w[k] = __ldg(bm1 + (c[k] >> 5));
             } else {
 #pragma unroll
-                for (int k = 0; k < 8; ++k) w[k] = (phases >> (8 + k) & 1u) ? __ldg(bm1 + (c[k] >> 5)) : 0u;
+                for (int k = 0; k < 8; ++k) w[k] = (live >> k & 1u) ? __ldg(bm1 + (c[k] >> 5)) : 0u;
             }
             uint32_t surv = 0; /* dead slots carry w = 0 */
 #pragma unroll
@@ -2482,6 +2501,29 @@ cudaError_t xgm_launch_merge(const double* gw, const uint32_t* gd, const XgmDevR
         if (e != cudaSuccess) return e;
     }
     xgm_merge_kernel<<<nq, 256, smem, s>>>(gw, gd, ginfo, part_w, part_d, part_info, nparts, nq, stride, k, out_w, out_d, out_n);
+    return cudaGetLastError();
+}
+
+/* ------------------------------------------------------------------ coarse bitmaps (index upload) */
+
+/* Coarse word g summarises fine words 8g .. 8g + 7 (one 256-docid group): bit 4k + j is set if byte j of fine word
+ * 8g + k is non-zero, i.e. bit (d >> 3) & 31 stands for docids d & ~7 .. (d & ~7) + 7. */
+__global__ void __launch_bounds__(256) xgm_coarse_kernel(const uint4* __restrict__ bm, size_t ncoarse, uint32_t* __restrict__ coarse) {
+    const size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= ncoarse) return;
+    const uint4 a = bm[2 * g], b = bm[2 * g + 1];
+    const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    uint32_t out = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) out |= ((w[k] >> (8 * j)) & 0xffu ? 1u : 0u) << (4 * k + j);
+    coarse[g] = out;
+}
+
+cudaError_t xgm_launch_coarse(const uint32_t* bitmaps, size_t ncoarse, uint32_t* coarse, cudaStream_t s) {
+    if (ncoarse == 0) return cudaSuccess;
+    xgm_coarse_kernel<<<(unsigned)((ncoarse + 255) / 256), 256, 0, s>>>(reinterpret_cast<const uint4*>(bitmaps), ncoarse, coarse);
     return cudaGetLastError();
 }
 
