@@ -192,7 +192,9 @@ typedef struct xgm_query {
     const uint32_t* wqf;         /* NULL → 1 each */
     uint32_t first, maxitems, check_at_least;   /* Enquire::get_mset arguments */
     const xgm_stats* stats;      /* NULL → local statistics */
-    double k1, k3, b, min_normlen; /* BM25Weight parameters; all 0 → defaults 1,1,0.5,0.5 (weight.h:665-667) */
+    double k1, k3, b, min_normlen; /* BM25Weight parameters; all 0 → defaults 1,1,0.5,0.5 (weight.h:665-667);
+                                      otherwise clamped as BM25Weight's constructor does: k1, k3 < 0 → 0,
+                                      b to [0, 1] (weight.h:639-646) */
     uint32_t filter, filter_slot;
     uint64_t range_lo, range_hi;
     uint32_t sort_by, sort_slot, sort_reverse, sort_use_max; /* sort_use_max: key = largest value of the slot */

@@ -566,8 +566,14 @@ static int list_contains(const uint32_t* d, uint32_t n, uint32_t did, uint32_t* 
     return lo < n && d[lo] == did;
 }
 
-int orc_match(const orc_index* ix, const orc_query* q, orc_mset* out) {
+int orc_match(const orc_index* ix, const orc_query* qin, orc_mset* out) {
     memset(out, 0, sizeof(*out));
+    /* BM25Weight's constructor, weight.h:639-646: k1, k3 < 0 become 0, b is clamped to [0, 1] */
+    orc_query qc = *qin;
+    if (qc.k1 < 0) qc.k1 = 0;
+    if (qc.k3 < 0) qc.k3 = 0;
+    if (qc.b < 0) qc.b = 0; else if (qc.b > 1) qc.b = 1;
+    const orc_query* q = &qc;
     uint32_t n = q->nterms;
     if (n == 0 || n > 64) return -1;
     /* Enquire::Internal::get_mset clamping, api/enquire.cc:420-426 */

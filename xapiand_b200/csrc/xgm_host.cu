@@ -1423,6 +1423,10 @@ static void term_weight(const xgm_index* ix, const xgm_query& q, const PlanTerms
 static xgm_status weigh_terms(const xgm_index* ix, const xgm_query& q, PlanTerms& t) {
     t.k1 = q.k1; t.k3 = q.k3; t.b = q.b; t.mnl = q.min_normlen;
     if (t.k1 == 0 && t.k3 == 0 && t.b == 0 && t.mnl == 0) { t.k1 = 1; t.k3 = 1; t.b = 0.5; t.mnl = 0.5; }
+    /* BM25Weight's constructor (weight.h:639-646): k1, k3 < 0 become 0 and b is clamped to [0, 1], so a caller's
+     * out-of-range value weighs as the reference weighs it.  The MaxScore bounds rely on it too: outside that range
+     * the length term k1 * (normlen * b + 1 - b) can be negative and a posting can outweigh get_maxpart. */
+    t.k1 = std::max(t.k1, 0.0); t.k3 = std::max(t.k3, 0.0); t.b = std::min(std::max(t.b, 0.0), 1.0);
     t.N = q.stats ? q.stats->collection_size : ix->doccount;
     const uint64_t tl = q.stats ? q.stats->total_length : ix->total_length;
     t.len_factor = 0;
