@@ -244,6 +244,81 @@ __device__ __forceinline__ uint32_t match_bucket(const XgmDevQuery* q, double w,
     return q->sort_reverse ? b : (XGM_NBINS - 1 - b);
 }
 
+/* b* and the match count rise under other warps' atomics while a launch runs: every read goes to memory */
+__device__ __forceinline__ uint32_t live_bstar(const XgmQState* st) {
+    return *reinterpret_cast<const volatile uint32_t*>(&st->bstar);
+}
+__device__ __forceinline__ uint32_t live_total(const XgmQState* st) {
+    return *reinterpret_cast<const volatile uint32_t*>(&st->total);
+}
+
+/* ---- MaxScore bounds (the parallel form of OrPostList's w_min checks, orpostlist.cc:113-155) */
+
+/* Only a query ranked by weight alone, with a top-k to fill, can drop a match by a bound on its weight. */
+__device__ __forceinline__ bool prunes_by_weight(const XgmDevQuery* q) {
+    return q->sort_by == 0 && q->topk != 0;
+}
+
+/* Bucket of an upper bound ub.  A bound adds get_maxpart values in leaf order while the weight it bounds is summed
+ * in the OrPostList tree's order, and the two round differently: the slack keeps a bound that a document attains
+ * from landing one bucket below the document's own weight. */
+__device__ __forceinline__ uint32_t bound_bucket(const XgmDevQuery* q, double ub) {
+    return match_bucket(q, ub * (1.0 + 1e-12), 0);
+}
+
+/* init + the get_maxpart bounds of the leaves whose bit is set in mask, added in ascending leaf order */
+__device__ __forceinline__ double maxpart_sum(const XgmDevQuery* q, uint32_t mask, double init) {
+    for (uint32_t i = 0; i < q->nterms; ++i)
+        if (mask >> i & 1u) init += q->terms[i].maxpart;
+    return init;
+}
+
+/* Bound on the weight of an owner leaf (termweight tw, get_maxpart maxpart) within one of its blocks (header word
+ * meta): its weight at the block's largest wdf in the shortest document, increasing in wdf and decreasing in length.
+ * A saturated header byte means a wdf of 255 or more, where only the leaf's own bound holds. */
+__device__ __forceinline__ double owner_block_bound(const XgmKernelParams& p, const XgmDevQuery* q, uint32_t meta,
+                                                    double tw, double maxpart) {
+    const uint32_t mw = XGM_HDR_MAXWDF(meta);
+    return mw == 255u ? maxpart : bm25_sumpart(tw, q, mw, p.doclen_lb);
+}
+
+/* MaxScore at work-item granularity: a document owned by leaf `drv` contains no rarer leaf, so its weight is bounded
+ * by the get_maxpart sum of leaves drv..n-1.  Once the top-k threshold b* is above that bound — and at least
+ * check_at_least matches have been counted, as ProtoMSet requires before min_weight may rise
+ * (protomset.h:185-194) — nothing the item owns can enter the MSet: it is skipped without decoding a block, and the
+ * query is marked as having skipped matches.  Work items are ordered rarest leaf first, so the frequent
+ * (low-weight) leaves, which hold most of the union, are usually skipped wholesale. */
+__device__ __forceinline__ bool skip_owned_item(const XgmKernelParams& p, const XgmDevQuery* q, uint32_t qi,
+                                                uint32_t drv, uint32_t lane) {
+    XgmQState* st = &p.qstate[qi];
+    const uint32_t bstar = live_bstar(st);
+    if (bstar == 0 || live_total(st) < q->check_at_least) return false;
+    if (bound_bucket(q, maxpart_sum(q, ~((1u << drv) - 1u), 0.0)) >= bstar) return false;
+    if (lane == 0) st->skipped = 1u;
+    return true;
+}
+
+/* ---- work lists: each kernel claims its items from work counter slot + pass (XGM_WC_*, xgm_device.h) */
+
+/* The second pass, when no query of the batch re-runs: the kernel has nothing to do. */
+__device__ __forceinline__ bool nothing_to_rerun(const XgmKernelParams& p) {
+    return p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0;
+}
+
+/* Claim the next of nitems work items of counter `slot` in this pass; false once they are all taken.  Warp-uniform. */
+__device__ __forceinline__ bool claim_item(const XgmKernelParams& p, uint32_t slot, uint32_t nitems, uint32_t lane,
+                                           uint32_t& item) {
+    uint32_t i = 0;
+    if (lane == 0) i = atomicAdd(p.work_counter + slot + p.pass, 1u);
+    item = __shfl_sync(FULL, i, 0);
+    return item < nitems;
+}
+
+/* Query qi runs in this pass: every query in the first, only those marked for re-running in the second. */
+__device__ __forceinline__ bool runs_this_pass(const XgmKernelParams& p, uint32_t qi) {
+    return p.pass == 0 || p.qstate[qi].rerun != 0;
+}
+
 /* A match whose weight is at least the running maximum: append it to the query's raise log (format.h) */
 __device__ __forceinline__ void log_raise(const XgmKernelParams& p, uint32_t qi, unsigned long long wb, uint32_t did, uint32_t subqs) {
     const uint32_t slot = atomicAdd(&p.qstate[qi].nraise, 1u);
@@ -251,6 +326,35 @@ __device__ __forceinline__ void log_raise(const XgmKernelParams& p, uint32_t qi,
         XgmRaise r;
         r.wbits = wb; r.docid = did; r.subqs = subqs;
         p.raise_log[(size_t)qi * XGM_RAISE_LOG + slot] = r;
+    }
+}
+
+/* Highest bin with at least topk stored matches at or above it → raise the query's pruning bucket.  Warp-converged
+ * call. */
+__device__ __noinline__ void raise_bstar_warp(const XgmDevQuery* q, XgmQState* st, const uint32_t* hist, uint32_t lane) {
+    const volatile uint32_t* vh = hist;
+    __threadfence();
+    uint32_t mine = 0;
+    for (int i = 0; i < XGM_NBINS / 32; ++i) mine += vh[lane * (XGM_NBINS / 32) + i];
+    /* suffix sum over lanes: sfx = sum of lanes >= lane */
+    uint32_t sfx = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        uint32_t t = __shfl_down_sync(FULL, sfx, o);
+        if ((int)lane + o < 32) sfx += t;
+    }
+    const uint32_t ok = __ballot_sync(FULL, sfx >= q->topk);
+    if (ok) {
+        const uint32_t L = 31 - __clz(ok);
+        if (lane == L) {
+            uint32_t cum = sfx - mine;
+            uint32_t nb = L * (XGM_NBINS / 32);
+            for (int i = XGM_NBINS / 32 - 1; i >= 0; --i) {
+                cum += vh[L * (XGM_NBINS / 32) + i];
+                if (cum >= q->topk) { nb = L * (XGM_NBINS / 32) + i; break; }
+            }
+            atomicMax(&st->bstar, nb);
+        }
     }
 }
 
@@ -277,7 +381,7 @@ __device__ __noinline__ void emit_matches_impl(const XgmKernelParams& p, const X
         mb = t > mb ? t : mb;
     }
     const uint32_t nall = __reduce_add_sync(FULL, __popc(alive));
-    const uint32_t bstar = *reinterpret_cast<volatile uint32_t*>(&st->bstar);
+    const uint32_t bstar = live_bstar(st);
     uint64_t key[4] = {0, 0, 0, 0};
     uint32_t bkt[4] = {0, 0, 0, 0};
     uint32_t keep = 0;
@@ -351,32 +455,8 @@ __device__ __noinline__ void emit_matches_impl(const XgmKernelParams& p, const X
     const uint32_t after = base + nkeep;
     /* (not before half of what the top-k kernel can rank is in use: small match sets stay unpruned, so
      * their known_matching_docs is reproduced exactly) */
-    if (p.pass == 0 && (base >> 8) != (after >> 8) && after >= q->topk && after >= p.keep_cap / 2) {
-        __threadfence();
-        const volatile uint32_t* vh = hist;
-        uint32_t mine = 0;
-        for (int i = 0; i < XGM_NBINS / 32; ++i) mine += vh[lane * (XGM_NBINS / 32) + i];
-        /* suffix sum over lanes: sfx = sum of lanes >= lane */
-        uint32_t sfx = mine;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t t = __shfl_down_sync(FULL, sfx, o);
-            if ((int)lane + o < 32) sfx += t;
-        }
-        const uint32_t ok = __ballot_sync(FULL, sfx >= q->topk);
-        if (ok) {
-            const uint32_t L = 31 - __clz(ok);
-            if (lane == L) {
-                uint32_t cum = sfx - mine;
-                uint32_t nb = L * (XGM_NBINS / 32);
-                for (int i = XGM_NBINS / 32 - 1; i >= 0; --i) {
-                    cum += vh[L * (XGM_NBINS / 32) + i];
-                    if (cum >= q->topk) { nb = L * (XGM_NBINS / 32) + i; break; }
-                }
-                atomicMax(&st->bstar, nb);
-            }
-        }
-    }
+    if (p.pass == 0 && (base >> 8) != (after >> 8) && after >= q->topk && after >= p.keep_cap / 2)
+        raise_bstar_warp(q, st, hist, lane);
 }
 
 /* count_only: matches already proven unable to reach the top-k (MaxScore bound below b*): they are
@@ -518,23 +598,43 @@ __device__ __noinline__ bool lookup_posting(const XgmKernelParams& p, const XgmD
 /* OrPostList::get_weight (matcher/orpostlist.cc:93-103): the tree over the leaves that hold the document, l, r or
  * l + r per node, evaluated as the postfix program q->prog built on the host (leaf >= 0, '+' = -1).  leaf(op, v)
  * returns whether leaf op holds the document and, if it does, sets v to the leaf's weight.  The result is only
- * defined when some leaf holds the document: the callers know whether one does. */
-template <class Leaf>
+ * defined when some leaf holds the document: the callers know whether one does.  DEPTH bounds the program's stack
+ * (at most one slot per leaf).  Up to a depth of 8 every slot is reached by static indexing, which keeps the stack
+ * in registers; deeper stacks are indexed dynamically and live in the local-memory frame. */
+template <int DEPTH, class Leaf>
 __device__ __forceinline__ double or_tree_weight(const XgmDevQuery* q, Leaf leaf) {
-    double stk[XGM_DEV_MAX_TERMS];
+    double stk[DEPTH];
+    auto set = [&](int s, double v) {
+        if constexpr (DEPTH > 8) {
+            stk[s] = v;
+        } else {
+#pragma unroll
+            for (int j = 0; j < DEPTH; ++j)
+                if (s == j) stk[j] = v;
+        }
+    };
+    auto get = [&](int s) {
+        if constexpr (DEPTH > 8) return stk[s];
+        double v = 0.0;
+#pragma unroll
+        for (int j = 0; j < DEPTH; ++j)
+            if (s == j) v = stk[j];
+        return v;
+    };
     uint32_t has = 0; /* bit s: stack slot s holds a value */
     int sp = 0;
     for (uint32_t i = 0; i < q->prog_len; ++i) {
         const int op = q->prog[i];
         if (op >= 0) {
-            if (leaf((uint32_t)op, stk[sp])) has |= 1u << sp;
+            double v;
+            if (leaf((uint32_t)op, v)) { set(sp, v); has |= 1u << sp; }
             else has &= ~(1u << sp);
             ++sp;
         } else {
             --sp;
             const bool hl = has >> (sp - 1) & 1u, hr = has >> sp & 1u;
-            if (hl && hr) stk[sp - 1] = __dadd_rn(stk[sp - 1], stk[sp]);
-            else if (hr) { stk[sp - 1] = stk[sp]; has |= 1u << (sp - 1); }
+            if (hl && hr) set(sp - 1, __dadd_rn(get(sp - 1), get(sp)));
+            else if (hr) { set(sp - 1, get(sp)); has |= 1u << (sp - 1); }
         }
     }
     return stk[0];
@@ -548,7 +648,7 @@ __device__ __noinline__ double maybe_weight(const XgmKernelParams& p, const XgmD
      * order ptxas gives xgm_and_bm3_kernel, which calls this function, a 176-byte frame and spills instead of 160 */
     uint32_t cnt = 0, wdf;
     const uint32_t base = q->nterms + q->nnot;
-    const double w = or_tree_weight(q, [&](uint32_t op, double& v) {
+    const double w = or_tree_weight<XGM_DEV_MAX_TERMS>(q, [&](uint32_t op, double& v) {
         const XgmDevTerm& t = q->terms[base + op];
         wdf = 0;
         if (!lookup_posting(p, t, d, &wdf)) return false;
@@ -570,7 +670,7 @@ struct __align__(16) AndScratch {
 
 /* The planner sends every AND whose lists but the driver all have bitmaps to xgm_and_bm3_kernel: here some list
  * has none, or the query has a single term. */
-__global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(XgmKernelParams p) {
+__global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(const __grid_constant__ XgmKernelParams p) {
     __shared__ AndScratch scratch[MATCH_WARPS];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     AndScratch& as = scratch[warp];
@@ -581,14 +681,11 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(XgmKernelP
     uint32_t phase = 0, dphase0 = 0, dphase1 = 0;
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
 
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return; /* nothing to re-run */
-    for (;;) {
-        uint32_t item = 0;
-        if (lane == 0) item = atomicAdd(p.work_counter + XGM_WC_AND + p.pass, 1u);
-        item = __shfl_sync(FULL, item, 0);
-        if (item >= p.nitems) break;
+    if (nothing_to_rerun(p)) return;
+    uint32_t item;
+    while (claim_item(p, XGM_WC_AND, p.nitems, lane, item)) {
         const XgmWorkItem wi = p.items[item];
-        if (p.pass != 0 && p.qstate[wi.query].rerun == 0) continue;
+        if (!runs_this_pass(p, wi.query)) continue;
         const XgmDevQuery* q = &p.queries[wi.query];
         const uint32_t nterms = q->nterms, nnot = q->nnot, nweighted = q->nweighted;
         /* lane j keeps list j's skip-table cursor (required lists, then the excluded ones of an OP_AND_NOT) */
@@ -770,36 +867,6 @@ static_assert(XGM_BM_RUN <= 16, "q1src keeps a query slot in 4 bits");
  * bitmap probes keep ~90 KB of L1 (51 KB per CTA would push the carve-out to 228 KB and leave the probes
  * almost no L1). */
 
-/* Highest bin with at least topk stored matches at or above it → raise the query's pruning bucket
- * (the warp-cooperative half of emit_matches_impl). */
-__device__ __noinline__ void raise_bstar_warp(const XgmKernelParams& p, uint32_t qi, uint32_t lane) {
-    const XgmDevQuery* q = &p.queries[qi];
-    XgmQState* st = &p.qstate[qi];
-    const volatile uint32_t* vh = p.hist + (size_t)qi * XGM_NBINS;
-    __threadfence();
-    uint32_t mine = 0;
-    for (int i = 0; i < XGM_NBINS / 32; ++i) mine += vh[lane * (XGM_NBINS / 32) + i];
-    uint32_t sfx = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t t = __shfl_down_sync(FULL, sfx, o);
-        if ((int)lane + o < 32) sfx += t;
-    }
-    const uint32_t ok = __ballot_sync(FULL, sfx >= q->topk);
-    if (ok) {
-        const uint32_t L = 31 - __clz(ok);
-        if (lane == L) {
-            uint32_t cum = sfx - mine;
-            uint32_t nb = L * (XGM_NBINS / 32);
-            for (int i = XGM_NBINS / 32 - 1; i >= 0; --i) {
-                cum += vh[L * (XGM_NBINS / 32) + i];
-                if (cum >= q->topk) { nb = L * (XGM_NBINS / 32) + i; break; }
-            }
-            atomicMax(&st->bstar, nb);
-        }
-    }
-}
-
 /* Per-lane emission of one match (lanes of a flush belong to different queries): count it, keep it unless
  * its bucket is already below the query's pruning bucket.  Warp-converged call. */
 __device__ __forceinline__ void emit_match_lanes(const XgmKernelParams& p, uint32_t lane, bool alive, uint32_t qi, double w,
@@ -824,8 +891,7 @@ __device__ __forceinline__ void emit_match_lanes(const XgmKernelParams& p, uint3
         }
         const uint64_t key = q->sort_by != 0 ? doc_sort_key(p, q, d) : 0ull;
         const uint32_t bkt = match_bucket(q, w, key);
-        const uint32_t bstar = *reinterpret_cast<volatile uint32_t*>(&st->bstar);
-        if (bkt >= bstar && q->topk != 0) {
+        if (bkt >= live_bstar(st) && q->topk != 0) {
             const uint32_t idx = atomicAdd(&st->stored, 1u);
             const uint64_t kv = q->sort_by != 0 ? key : (uint64_t)aux;
             if (p.pass == 0) {
@@ -848,7 +914,8 @@ __device__ __forceinline__ void emit_match_lanes(const XgmKernelParams& p, uint3
     while (m) {
         const uint32_t l = (uint32_t)__ffs(m) - 1u;
         m &= m - 1u;
-        raise_bstar_warp(p, __shfl_sync(FULL, qi, l), lane);
+        const uint32_t rq = __shfl_sync(FULL, qi, l);
+        raise_bstar_warp(&p.queries[rq], &p.qstate[rq], p.hist + (size_t)rq * XGM_NBINS, lane);
     }
 }
 
@@ -868,7 +935,7 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, 4) xgm_and_bm3_kernel(const __
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
     const uint32_t stage_base = smem_u32(ws.dstage[0]);
     const uint32_t bar_base = stage_base + (uint32_t)offsetof(Bm3Scratch, dbar);
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return;
+    if (nothing_to_rerun(p)) return;
     const uint32_t nitems_bm = p.nitems_bm_dev ? __ldg(p.nitems_bm_dev) : p.nitems_bm;
     uint32_t qn1 = 0, qn2 = 0; /* warp-uniform queue lengths */
     bool done = false;
@@ -970,14 +1037,12 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, 4) xgm_and_bm3_kernel(const __
         if (done) break;
         /* ---- next work item ---- */
         if (item_end) {
-            uint32_t item = 0;
-            if (lane == 0) item = atomicAdd(p.work_counter + XGM_WC_AND_BM + p.pass, 1u);
-            item = __shfl_sync(FULL, item, 0);
-            if (item >= nitems_bm) { done = true; continue; }
+            uint32_t item;
+            if (!claim_item(p, XGM_WC_AND_BM, nitems_bm, lane, item)) { done = true; continue; }
             const XgmWorkItem wi = p.items_bm[item];
             const uint32_t n = p.bm_segs ? wi.pad : 1u;
             slot_q = lane >= n ? 0u : p.bm_segs ? p.bm_segs[wi.query + lane].query : wi.query;
-            const bool take = lane < n && (p.pass == 0 || p.qstate[slot_q].rerun != 0);
+            const bool take = lane < n && runs_this_pass(p, slot_q);
             run_bits = __ballot_sync(FULL, take);
             if (run_bits == 0) continue; /* second pass: no query of the run re-runs */
             slot_bm = take ? p.queries[slot_q].terms[1].bm_off | p.queries[slot_q].probe_coarse : 0ull;
@@ -1139,7 +1204,7 @@ struct __align__(16) OrScratch {
  * MaxScore pruning, the parallel form of OrPostList's w_min checks (orpostlist.cc:113-155): a document
  * whose present leaves cannot add up to the current top-k threshold (sum of their get_maxpart bounds
  * falls in a bucket below b*) is counted as a match but neither scored nor stored. */
-__global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(XgmKernelParams p) {
+__global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(const __grid_constant__ XgmKernelParams p) {
     __shared__ OrScratch scratch[OR_WARPS];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     OrScratch& os = scratch[warp];
@@ -1150,14 +1215,11 @@ __global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(XgmKernelParams p
     uint32_t phase = 0;
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
 
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return;
-    for (;;) {
-        uint32_t item = 0;
-        if (lane == 0) item = atomicAdd(p.work_counter + XGM_WC_OR + p.pass, 1u);
-        item = __shfl_sync(FULL, item, 0);
-        if (item >= p.nitems_or) break;
+    if (nothing_to_rerun(p)) return;
+    uint32_t item;
+    while (claim_item(p, XGM_WC_OR, p.nitems_or, lane, item)) {
         const XgmWorkItem wi = p.items_or[item];
-        if (p.pass != 0 && p.qstate[wi.query].rerun == 0) continue;
+        if (!runs_this_pass(p, wi.query)) continue;
         const XgmDevQuery* q = &p.queries[wi.query];
         if (q->or_fast != XGM_OR_FAST_GENERAL) continue; /* answered by xgm_or3_kernel */
         const uint32_t nterms = q->nterms;
@@ -1168,27 +1230,8 @@ __global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(XgmKernelParams p
             my_nblk = q->terms[lane].nblocks;
         }
         const uint32_t drv_begin = __shfl_sync(FULL, my_begin, drv);
-        const bool can_prune = (q->sort_by == 0) && (q->topk != 0);
-
-        /* MaxScore at work-item granularity: a document owned by leaf `drv` contains no rarer leaf, so its
-         * weight is bounded by the get_maxpart sum of leaves drv..n-1.  Once the top-k threshold b* is above
-         * that bound — and at least check_at_least matches have been counted, as ProtoMSet requires before
-         * min_weight may rise (protomset.h:185-194) — nothing this item owns can enter the MSet: skip it
-         * without decoding a block.  Work items are ordered rarest leaf first, so the frequent (low-weight)
-         * leaves, which hold most of the union, are usually skipped wholesale. */
-        if (can_prune) {
-            const XgmQState* st = &p.qstate[wi.query];
-            const uint32_t bstar = *reinterpret_cast<const volatile uint32_t*>(&st->bstar);
-            if (bstar != 0 && *reinterpret_cast<const volatile uint32_t*>(&st->total) >= q->check_at_least) {
-                double ub = 0.0;
-                for (uint32_t i = drv; i < nterms; ++i) ub += q->terms[i].maxpart;
-                ub *= 1.0 + 1e-12;
-                if (match_bucket(q, ub, 0) < bstar) {
-                    if (lane == 0) p.qstate[wi.query].skipped = 1u;
-                    continue;
-                }
-            }
-        }
+        const bool can_prune = prunes_by_weight(q);
+        if (can_prune && skip_owned_item(p, q, wi.query, drv, lane)) continue;
 
         for (uint32_t db = wi.b0; db < wi.b1; ++db) {
             const XgmBlockHdr dh = hdr[drv_begin + db];
@@ -1260,18 +1303,11 @@ __global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(XgmKernelParams p
             /* MaxScore: can the leaves present reach the current threshold at all? */
             uint32_t skip = 0;
             if (can_prune) {
-                const uint32_t bstar = *reinterpret_cast<volatile uint32_t*>(&p.qstate[wi.query].bstar);
+                const uint32_t bstar = live_bstar(&p.qstate[wi.query]);
                 if (bstar != 0) {
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        if (owned >> k & 1u) {
-                            double ub = 0.0;
-                            for (uint32_t i = 0; i < nterms; ++i)
-                                if (present[k] >> i & 1u) ub += q->terms[i].maxpart;
-                            ub *= 1.0 + 1e-12; /* the bound and the tree-order sum round differently */
-                            if (match_bucket(q, ub, 0) < bstar) skip |= 1u << k;
-                        }
-                    }
+                    for (int k = 0; k < 4; ++k)
+                        if ((owned >> k & 1u) && bound_bucket(q, maxpart_sum(q, present[k], 0.0)) < bstar) skip |= 1u << k;
                 }
             }
             /* weight = fold of the tree over the leaves present (OrPostList::get_weight, orpostlist.cc:93-103) */
@@ -1282,7 +1318,7 @@ __global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(XgmKernelParams p
                 if ((owned & ~skip) >> k & 1u) {
                     const uint32_t d = c[k];
                     const uint32_t dlen = __ldg(&p.doclen[d]);
-                    acc[k] = or_tree_weight(q, [&](uint32_t op, double& v) {
+                    acc[k] = or_tree_weight<XGM_DEV_MAX_TERMS>(q, [&](uint32_t op, double& v) {
                         if (!(present[k] >> op & 1u)) return false;
                         uint32_t tf;
                         if (op == drv) {
@@ -1306,54 +1342,29 @@ __global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(XgmKernelParams p
     }
 }
 
-/* Weight of document d of an OR query = fold of the reference's OrPostList tree over the leaves present
- * (OrPostList::get_weight, orpostlist.cc:93-103; presence mask pm over leaf positions).  The wdf of leaf `drv`
- * (the owner, if any: drv < nterms) comes from position pos of the block whose header is hdr[src]; every other
- * leaf is looked up through its rank directory.  At most OR3_MAX_LEAVES leaves: the stack stays in registers. */
+/* Weight of document d of an OR query of at most OR3_MAX_LEAVES leaves (presence mask pm over leaf positions): the
+ * OrPostList tree fold (or_tree_weight) with its stack in registers.  The wdf of leaf `drv` (the owner, if any:
+ * drv < nterms) comes from position pos of the block whose header is hdr[src]; every other leaf is looked up through
+ * its rank directory. */
 #define OR3_MAX_LEAVES 5
 __device__ __forceinline__ double or_score_doc(const XgmKernelParams& p, const XgmDevQuery* mq, uint32_t d, uint32_t pm,
                                                uint32_t drv, uint32_t src, uint32_t pos) {
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
     const uint32_t dlen = __ldg(&p.doclen[d]);
-    double stk[OR3_MAX_LEAVES + 1];
-    uint32_t has = 0;
-    int sp = 0;
-    const uint32_t plen = mq->prog_len;
-    for (uint32_t i = 0; i < plen; ++i) {
-        const int op = mq->prog[i];
-        if (op >= 0) {
-            if (pm >> op & 1u) {
-                uint32_t tf;
-                if ((uint32_t)op == drv) {
-                    const XgmBlockHdr hh = hdr[src];
-                    tf = unpack_gl(p.tfs, hh.tf_off, pos, XGM_HDR_TF_BITS(hh.meta));
-                } else {
-                    const uint32_t r = bitmap_rank(p, mq->terms[op], d);
-                    const XgmBlockHdr bh = hdr[mq->terms[op].blk_begin + (r >> 7)];
-                    tf = unpack_gl(p.tfs, bh.tf_off, r & 127u, XGM_HDR_TF_BITS(bh.meta));
-                }
-                const double v = bm25_sumpart(mq->terms[op].termweight, mq, tf, dlen);
-                /* static indexing keeps the stack in registers */
-                if (sp == 0) stk[0] = v; else if (sp == 1) stk[1] = v; else if (sp == 2) stk[2] = v;
-                else if (sp == 3) stk[3] = v; else if (sp == 4) stk[4] = v; else stk[5] = v;
-                has |= 1u << sp;
-            } else {
-                has &= ~(1u << sp);
-            }
-            ++sp;
+    return or_tree_weight<OR3_MAX_LEAVES>(mq, [&](uint32_t op, double& v) {
+        if (!(pm >> op & 1u)) return false;
+        uint32_t tf;
+        if (op == drv) {
+            const XgmBlockHdr hh = hdr[src];
+            tf = unpack_gl(p.tfs, hh.tf_off, pos, XGM_HDR_TF_BITS(hh.meta));
         } else {
-            --sp;
-            const bool hl = has >> (sp - 1) & 1u, hr = has >> sp & 1u;
-            const double r = sp == 1 ? stk[1] : sp == 2 ? stk[2] : sp == 3 ? stk[3] : sp == 4 ? stk[4] : stk[5];
-            const double l = sp == 1 ? stk[0] : sp == 2 ? stk[1] : sp == 3 ? stk[2] : sp == 4 ? stk[3] : stk[4];
-            double v = l;
-            if (hl && hr) v = __dadd_rn(l, r);
-            else if (hr) { v = r; has |= 1u << (sp - 1); }
-            if (sp == 1) stk[0] = v; else if (sp == 2) stk[1] = v; else if (sp == 3) stk[2] = v;
-            else if (sp == 4) stk[3] = v; else stk[4] = v;
+            const uint32_t r = bitmap_rank(p, mq->terms[op], d);
+            const XgmBlockHdr bh = hdr[mq->terms[op].blk_begin + (r >> 7)];
+            tf = unpack_gl(p.tfs, bh.tf_off, r & 127u, XGM_HDR_TF_BITS(bh.meta));
         }
-    }
-    return stk[0];
+        v = bm25_sumpart(mq->terms[op].termweight, mq, tf, dlen);
+        return true;
+    });
 }
 
 /* ------------------------------------------------------------------ OR kernel, bitmap leaves + queued scoring */
@@ -1395,7 +1406,7 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, 3) xgm_or3_kernel(const __grid
     const XgmBlockHdr* __restrict__ hdr = p.hdr;
     const uint32_t stage_base = smem_u32(ws.dstage[0]);
     const uint32_t bar_base = stage_base + (uint32_t)offsetof(Or3Scratch, dbar);
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return;
+    if (nothing_to_rerun(p)) return;
     uint32_t qn = 0; /* warp-uniform queue length */
     bool done = false;
     /* current work item: blocks [db, it_b1) of leaf it_drv of query it_query are left */
@@ -1437,14 +1448,12 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, 3) xgm_or3_kernel(const __grid
                 /* before the other leaves are looked up: the owner's exact weight plus the bounds of the others
                  * already decides most documents (MaxScore at its finest grain) */
                 const XgmDevQuery* mq = &p.queries[qi];
-                const uint32_t bstar = (mq->sort_by == 0 && mq->topk != 0) ? *reinterpret_cast<volatile uint32_t*>(&p.qstate[qi].bstar) : 0u;
+                const uint32_t bstar = prunes_by_weight(mq) ? live_bstar(&p.qstate[qi]) : 0u;
                 if (bstar != 0) {
                     const XgmBlockHdr hh = hdr[src];
                     const uint32_t tf = unpack_gl(p.tfs, hh.tf_off, pos, XGM_HDR_TF_BITS(hh.meta));
-                    double ub = bm25_sumpart(mq->terms[drv].termweight, mq, tf, __ldg(&p.doclen[d]));
-                    for (uint32_t i = 0; i < mq->nterms; ++i)
-                        if ((pm >> i & 1u) && i != drv) ub += mq->terms[i].maxpart;
-                    if (match_bucket(mq, ub * (1.0 + 1e-12), 0) < bstar) score = false;
+                    const double own = bm25_sumpart(mq->terms[drv].termweight, mq, tf, __ldg(&p.doclen[d]));
+                    if (bound_bucket(mq, maxpart_sum(mq, pm & ~(1u << drv), own)) < bstar) score = false;
                 }
             }
             if (score) acc = or_score_doc(p, &p.queries[qi], d, pm, drv, src, pos);
@@ -1460,32 +1469,22 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, 3) xgm_or3_kernel(const __grid
                 if (lane == 0 && t && p.pass == 0) atomicAdd(&p.qstate[it_query].total, t);
                 total_acc = 0; it_b1 = 0; db = 0;
             }
-            uint32_t item = 0;
-            if (lane == 0) item = atomicAdd(p.work_counter + (PHASE ? XGM_WC_OR3_SINGLE : XGM_WC_OR3) + p.pass, 1u);
-            item = __shfl_sync(FULL, item, 0);
-            if (item >= p.nitems_or) { done = true; continue; }
+            uint32_t item;
+            if (!claim_item(p, PHASE ? XGM_WC_OR3_SINGLE : XGM_WC_OR3, p.nitems_or, lane, item)) { done = true; continue; }
             const XgmWorkItem wi = p.items_or[item];
-            if (p.pass != 0 && p.qstate[wi.query].rerun == 0) continue;
+            if (!runs_this_pass(p, wi.query)) continue;
             q = &p.queries[wi.query];
             if (q->or_fast != (PHASE ? XGM_OR_FAST_TILE : XGM_OR_FAST_OR3)) continue; /* another kernel's query */
             nterms = q->nterms;
             it_drv = wi.pad;
-            can_prune = (q->sort_by == 0) && (q->topk != 0);
-            /* MaxScore at work-item granularity (see xgm_or_kernel): nothing this item owns can reach the top-k */
+            can_prune = prunes_by_weight(q);
             if (can_prune) {
-                const XgmQState* st = &p.qstate[wi.query];
-                const uint32_t bstar = *reinterpret_cast<const volatile uint32_t*>(&st->bstar);
                 if (PHASE) {
                     /* only single-leaf documents are left: none of this leaf can reach the threshold */
-                    if (bstar != 0 && match_bucket(q, q->terms[it_drv].maxpart * (1.0 + 1e-12), 0) < bstar) continue;
-                } else if (bstar != 0 && *reinterpret_cast<const volatile uint32_t*>(&st->total) >= q->check_at_least) {
-                    double ub = 0.0;
-                    for (uint32_t i = it_drv; i < nterms; ++i) ub += q->terms[i].maxpart;
-                    ub *= 1.0 + 1e-12;
-                    if (match_bucket(q, ub, 0) < bstar) {
-                        if (lane == 0) p.qstate[wi.query].skipped = 1u;
-                        continue;
-                    }
+                    const uint32_t bstar = live_bstar(&p.qstate[wi.query]);
+                    if (bstar != 0 && bound_bucket(q, q->terms[it_drv].maxpart) < bstar) continue;
+                } else if (skip_owned_item(p, q, wi.query, it_drv, lane)) {
+                    continue;
                 }
             }
             it_query = wi.query; it_b1 = wi.b1; db = wi.b0;
@@ -1494,14 +1493,9 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, 3) xgm_or3_kernel(const __grid
             for (int j = 0; j < OR3_MAX_LEAVES; ++j) bmp[j] = p.bitmaps + ((uint32_t)j < nterms ? q->terms[j].bm_off : 0ull);
             /* lane m holds, for presence mask m, the sum of the get_maxpart bounds of the leaves other than the
              * owner; the owner's own bound is per block (its largest wdf is in the header) */
-            {
-                double ub = 0.0;
-                for (uint32_t i = 0; i < nterms; ++i)
-                    if ((lane >> i & 1u) && i != it_drv) ub += q->terms[i].maxpart;
-                others = ub;
-                drv_tw = q->terms[it_drv].termweight;
-                drv_maxpart = q->terms[it_drv].maxpart;
-            }
+            others = maxpart_sum(q, lane & ~(1u << it_drv), 0.0);
+            drv_tw = q->terms[it_drv].termweight;
+            drv_maxpart = q->terms[it_drv].maxpart;
             for (uint32_t b = db; b < it_b1 && b < db + 3; ++b) issue(b);
             continue;
         }
@@ -1513,12 +1507,8 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, 3) xgm_or3_kernel(const __grid
             if (bits) { mbar_wait_a(bar_base + cur * 8u, (phases >> cur) & 1u); phases ^= 1u << cur; }
             if (PHASE) {
                 /* a block whose best possible single-leaf document is below the threshold is skipped whole */
-                const uint32_t bs = *reinterpret_cast<volatile uint32_t*>(&p.qstate[it_query].bstar);
-                if (bs != 0) {
-                    const uint32_t mw = XGM_HDR_MAXWDF(h.w);
-                    const double own = mw == 255u ? drv_maxpart : bm25_sumpart(drv_tw, q, mw, p.doclen_lb);
-                    if (match_bucket(q, own * (1.0 + 1e-12), 0) < bs) { ++db; continue; }
-                }
+                const uint32_t bs = live_bstar(&p.qstate[it_query]);
+                if (bs != 0 && bound_bucket(q, owner_block_bound(p, q, h.w, drv_tw, drv_maxpart)) < bs) { ++db; continue; }
             }
             uint32_t c[4];
             decode_docids(ws.dstage[cur], bits, h.x, lane, c);
@@ -1537,15 +1527,10 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, 3) xgm_or3_kernel(const __grid
                 }
             }
             const uint32_t rarer = (1u << it_drv) - 1u;
-            const uint32_t bstar = can_prune ? *reinterpret_cast<volatile uint32_t*>(&p.qstate[it_query].bstar) : 0u;
-            /* pruning bucket of every presence mask for THIS block: the owner contributes at most its weight at
-             * the block's largest wdf and the shortest document (increasing in wdf, decreasing in length) */
+            const uint32_t bstar = can_prune ? live_bstar(&p.qstate[it_query]) : 0u;
+            /* pruning bucket of every presence mask for THIS block: the owner's bound within the block plus the others' */
             uint32_t ubbkt = XGM_NBINS;
-            if (bstar != 0) {
-                const uint32_t mw = XGM_HDR_MAXWDF(h.w);
-                const double own = mw == 255u ? drv_maxpart : bm25_sumpart(drv_tw, q, mw, p.doclen_lb);
-                ubbkt = match_bucket(q, (own + others) * (1.0 + 1e-12), 0);
-            }
+            if (bstar != 0) ubbkt = bound_bucket(q, owner_block_bound(p, q, h.w, drv_tw, drv_maxpart) + others);
             uint32_t cand = 0;
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
@@ -1634,7 +1619,7 @@ __global__ void __launch_bounds__(TILE_WARPS * 32, 4) xgm_or_tile_kernel(const _
     __shared__ TileScratch scratch[TILE_WARPS];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     TileScratch& ws = scratch[warp];
-    if (p.pass != 0 && *reinterpret_cast<volatile uint32_t*>(p.work_counter + XGM_WC_RERUN) == 0) return;
+    if (nothing_to_rerun(p)) return;
     const uint32_t nwords = (p.lastdocid >> 5) + 1u;
     const uint32_t items_per_q = (nwords + 32u * TILE_ITERS - 1u) / (32u * TILE_ITERS);
     const uint32_t nitems = items_per_q * p.ntileq;
@@ -1652,13 +1637,10 @@ __global__ void __launch_bounds__(TILE_WARPS * 32, 4) xgm_or_tile_kernel(const _
         __syncwarp();
     };
 
-    for (;;) {
-        uint32_t item = 0;
-        if (lane == 0) item = atomicAdd(p.work_counter + XGM_WC_TILE + p.pass, 1u);
-        item = __shfl_sync(FULL, item, 0);
-        if (item >= nitems) break;
+    uint32_t item;
+    while (claim_item(p, XGM_WC_TILE, nitems, lane, item)) {
         const uint32_t tile = item / p.ntileq, qi = __ldg(p.tileq + (item - tile * p.ntileq));
-        if (p.pass != 0 && p.qstate[qi].rerun == 0) continue;
+        if (!runs_this_pass(p, qi)) continue;
         const XgmDevQuery* q = &p.queries[qi];
         const uint32_t nterms = q->nterms;
         /* the loads carry no per-leaf predicate: a missing leaf re-reads leaf 0's word (an L1 hit) and is masked */
@@ -1670,13 +1652,7 @@ __global__ void __launch_bounds__(TILE_WARPS * 32, 4) xgm_or_tile_kernel(const _
             lm[j] = (uint32_t)j < nterms ? 0xffffffffu : 0u;
         }
         /* lane m: pruning bucket of presence mask m (sum of the get_maxpart bounds of its leaves) */
-        uint32_t ubbkt;
-        {
-            double ub = 0.0;
-            for (uint32_t i = 0; i < nterms; ++i)
-                if (lane >> i & 1u) ub += q->terms[i].maxpart;
-            ubbkt = match_bucket(q, ub * (1.0 + 1e-12), 0);
-        }
+        const uint32_t ubbkt = bound_bucket(q, maxpart_sum(q, lane, 0.0));
         uint32_t total_acc = 0;
         const uint32_t w0 = tile * (32u * TILE_ITERS);
         const uint32_t iters = min((uint32_t)TILE_ITERS, (nwords - w0 + 31u) >> 5);
@@ -1703,7 +1679,7 @@ __global__ void __launch_bounds__(TILE_WARPS * 32, 4) xgm_or_tile_kernel(const _
             total_acc += (uint32_t)__popc(one);
             uint32_t cand = two;
             if (__any_sync(FULL, cand != 0)) {
-                const uint32_t bstar = *reinterpret_cast<volatile uint32_t*>(&p.qstate[qi].bstar);
+                const uint32_t bstar = live_bstar(&p.qstate[qi]);
                 do { /* one document per lane and round */
                     const bool has = cand != 0;
                     const uint32_t bit = has ? (uint32_t)__ffs(cand) - 1u : 0u;
