@@ -329,144 +329,112 @@ __device__ __forceinline__ void log_raise(const XgmKernelParams& p, uint32_t qi,
     }
 }
 
+/* Highest bin b whose bins [b, XGM_NBINS) of histogram h hold at least `want` entries, i.e. the bin of the want-th
+ * highest entry; 0 when the whole histogram holds fewer, which prunes nothing either.  32 bins per lane, a suffix scan
+ * over the lanes, then a walk inside the one lane's bins.  Every lane gets the result.  Warp-converged call.  The reads
+ * are volatile: other warps are still adding to a match kernel's histogram. */
+__device__ __forceinline__ uint32_t bin_of_rank(const volatile uint32_t* h, uint32_t want, uint32_t lane) {
+    constexpr int per = XGM_NBINS / 32;
+    uint32_t mine = 0;
+    for (int i = 0; i < per; ++i) mine += h[lane * per + i];
+    uint32_t sfx = mine; /* entries in the bins of lanes >= lane */
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_down_sync(FULL, sfx, o);
+        if ((int)lane + o < 32) sfx += t;
+    }
+    const uint32_t ok = __ballot_sync(FULL, sfx >= want);
+    if (ok == 0) return 0;
+    const uint32_t L = 31u - (uint32_t)__clz(ok); /* highest lane whose suffix reaches `want` */
+    uint32_t b = L * per;
+    if (lane == L) {
+        /* a bounded loop: written as a while loop, this walk costs xgm_or3_kernel two registers (via raise_bstar_warp) */
+        uint32_t cum = sfx - mine;
+        for (int i = per - 1; i >= 0; --i) {
+            cum += h[L * per + i];
+            if (cum >= want) { b = L * per + i; break; }
+        }
+    }
+    return __shfl_sync(FULL, b, L);
+}
+
 /* Highest bin with at least topk stored matches at or above it → raise the query's pruning bucket.  Warp-converged
  * call. */
 __device__ __noinline__ void raise_bstar_warp(const XgmDevQuery* q, XgmQState* st, const uint32_t* hist, uint32_t lane) {
-    const volatile uint32_t* vh = hist;
     __threadfence();
-    uint32_t mine = 0;
-    for (int i = 0; i < XGM_NBINS / 32; ++i) mine += vh[lane * (XGM_NBINS / 32) + i];
-    /* suffix sum over lanes: sfx = sum of lanes >= lane */
-    uint32_t sfx = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t t = __shfl_down_sync(FULL, sfx, o);
-        if ((int)lane + o < 32) sfx += t;
-    }
-    const uint32_t ok = __ballot_sync(FULL, sfx >= q->topk);
-    if (ok) {
-        const uint32_t L = 31 - __clz(ok);
-        if (lane == L) {
-            uint32_t cum = sfx - mine;
-            uint32_t nb = L * (XGM_NBINS / 32);
-            for (int i = XGM_NBINS / 32 - 1; i >= 0; --i) {
-                cum += vh[L * (XGM_NBINS / 32) + i];
-                if (cum >= q->topk) { nb = L * (XGM_NBINS / 32) + i; break; }
-            }
-            atomicMax(&st->bstar, nb);
-        }
-    }
+    const uint32_t nb = bin_of_rank(hist, q->topk, lane);
+    if (lane == 0 && nb != 0) atomicMax(&st->bstar, nb);
 }
 
-/* Warp-wide: lanes hold up to 4 matches each (mask `alive`), weight acc[k], docid c[k], aux[k]
- * (number of matching leaves). Counts every match, keeps those not yet prunable. */
-__device__ __noinline__ void emit_matches_impl(const XgmKernelParams& p, const XgmDevQuery* q, uint32_t qi, uint32_t lane,
-                                              uint32_t alive, double a0, double a1, double a2, double a3, uint32_t c0,
-                                              uint32_t c1, uint32_t c2, uint32_t c3, uint32_t x0, uint32_t x1,
-                                              uint32_t x2, uint32_t x3, uint32_t count_only) {
-    const double acc[4] = {a0, a1, a2, a3};
-    const uint32_t c[4] = {c0, c1, c2, c3};
-    const uint32_t aux[4] = {x0, x1, x2, x3};
-    XgmQState* st = &p.qstate[qi];
-    uint32_t* hist = p.hist + (size_t)qi * XGM_NBINS;
-    /* exact match count and best weight over ALL matches (ProtoMSet::update_max_weight, protomset.h:174-183) */
-    double lmax = 0.0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-        if ((alive >> k & 1u) && acc[k] > lmax) lmax = acc[k];
-    unsigned long long mb = (unsigned long long)__double_as_longlong(lmax);
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) {
-        unsigned long long t = __shfl_xor_sync(FULL, mb, o);
-        mb = t > mb ? t : mb;
+/* Whether `stored` matches of query q are enough to raise its b*.  An OR whose union comes from the bitmap kernels
+ * (or_fast OR3 or TILE) raises from topk on.  AND queries and the general OR route wait until half of what the top-k
+ * kernel can rank is in use: small match sets on those routes stay unpruned, so their known_matching_docs stays
+ * exact. */
+__device__ __forceinline__ bool may_raise_bstar(const XgmKernelParams& p, const XgmDevQuery* q, uint32_t stored) {
+    const bool bitmap_or = q->route == XGM_ROUTE_OR && q->or_fast != XGM_OR_FAST_GENERAL;
+    return stored >= q->topk && (bitmap_or || stored >= p.keep_cap / 2);
+}
+
+/* Add the lanes' counts n to query qi's exact match count, in the first pass: one atomic per warp.  Warp-converged
+ * call. */
+__device__ __forceinline__ void count_matches(const XgmKernelParams& p, uint32_t qi, uint32_t n, uint32_t lane) {
+    const uint32_t t = __reduce_add_sync(FULL, n);
+    if (lane == 0 && t && p.pass == 0) atomicAdd(&p.qstate[qi].total, t);
+}
+
+/* The emission of a match, one per lane (lanes of one call may belong to different queries): count it (unless the
+ * caller counts with count_matches), raise the query's best weight and log the raise, and keep it unless its bucket is
+ * already below the query's pruning bucket: in the first pass in the match buffer and the histogram, in the second in
+ * the query's slice of the pool.  Warp-converged call. */
+__device__ __forceinline__ void emit_match_lanes(const XgmKernelParams& p, uint32_t lane, bool alive, uint32_t qi, double w,
+                                                 uint32_t d, uint32_t aux, bool count = true) {
+    bool crossed = false;
+    /* A query with 10^5..10^6 matches would otherwise send every one of them to the same two words (total, maxw):
+     * same-address atomics serialise in L2 and one such query doubled the launch time of a 4096-query batch.  The
+     * lanes of one query are counted by their lowest lane, and maxw — which only rises — is read first. */
+    if (p.pass == 0 && count) {
+        const uint32_t grp = __match_any_sync(FULL, alive ? qi : 0xffffffffu);
+        if (alive && lane == (uint32_t)__ffs(grp) - 1u) atomicAdd(&p.qstate[qi].total, (uint32_t)__popc(grp));
     }
-    const uint32_t nall = __reduce_add_sync(FULL, __popc(alive));
-    const uint32_t bstar = live_bstar(st);
-    uint64_t key[4] = {0, 0, 0, 0};
-    uint32_t bkt[4] = {0, 0, 0, 0};
-    uint32_t keep = 0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        if (alive >> k & 1u) {
-            if (q->sort_by != 0) key[k] = doc_sort_key(p, q, c[k]);
-            bkt[k] = match_bucket(q, acc[k], key[k]);
-            if (bkt[k] >= bstar && q->topk != 0 && !(count_only >> k & 1u)) keep |= 1u << k;
-        }
-    }
-    const uint32_t n = __popc(keep);
-    uint32_t incl = n;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t t = __shfl_up_sync(FULL, incl, o);
-        if ((int)lane >= o) incl += t;
-    }
-    const uint32_t nkeep = __shfl_sync(FULL, incl, 31);
-    uint32_t base = 0;
-    unsigned long long oldmax = ~0ull;
-    if (lane == 0) {
+    if (alive) {
+        const XgmDevQuery* q = &p.queries[qi];
+        XgmQState* st = &p.qstate[qi];
         if (p.pass == 0) {
-            atomicAdd(&st->total, nall);
-            oldmax = atomicMax(&st->maxw, mb);
+            /* best weight over all matches (ProtoMSet::update_max_weight, protomset.h:174-183) */
+            const unsigned long long wb = (unsigned long long)__double_as_longlong(w);
+            if (wb >= *reinterpret_cast<volatile unsigned long long*>(&st->maxw)) {
+                const unsigned long long oldmax = atomicMax(&st->maxw, wb);
+                if (q->log_raises && wb >= oldmax) log_raise(p, qi, wb, d, aux);
+            }
         }
-        if (nkeep) base = atomicAdd(&st->stored, nkeep);
-    }
-    base = __shfl_sync(FULL, base, 0);
-    if (q->log_raises && p.pass == 0) {
-        oldmax = __shfl_sync(FULL, oldmax, 0);
-        if (mb >= oldmax) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                if ((alive >> k & 1u) && (unsigned long long)__double_as_longlong(acc[k]) == mb) log_raise(p, qi, mb, c[k], aux[k]);
-        }
-    }
-    if (nkeep == 0) return;
-    uint32_t idx = base + (incl - n);
-    if (p.pass == 0) {
-        const size_t qoff = (size_t)qi * p.match_cap;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            if (keep >> k & 1u) {
-                atomicAdd(&hist[bkt[k]], 1u);
+        const uint64_t key = q->sort_by != 0 ? doc_sort_key(p, q, d) : 0ull;
+        const uint32_t bkt = match_bucket(q, w, key);
+        if (bkt >= live_bstar(st) && q->topk != 0) {
+            const uint32_t idx = atomicAdd(&st->stored, 1u);
+            const uint64_t kv = q->sort_by != 0 ? key : (uint64_t)aux;
+            if (p.pass == 0) {
+                atomicAdd(p.hist + (size_t)qi * XGM_NBINS + bkt, 1u);
                 if (idx < p.match_cap) {
-                    p.match_w[qoff + idx] = acc[k];
-                    p.match_d[qoff + idx] = c[k];
-                    p.match_k[qoff + idx] = q->sort_by != 0 ? key[k] : (uint64_t)aux[k];
+                    const size_t o = (size_t)qi * p.match_cap + idx;
+                    p.match_w[o] = w; p.match_d[o] = d; p.match_k[o] = kv;
                 }
-                ++idx;
-            }
-        }
-    } else {
-        /* second pass: every match at or above the exact b* goes to the query's slice of the pool */
-        const size_t poff = st->pool_off;
-        const uint32_t pcap = st->pool_cap;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            if (keep >> k & 1u) {
-                if (idx < pcap) {
-                    p.pool_w[poff + idx] = acc[k];
-                    p.pool_d[poff + idx] = c[k];
-                    p.pool_k[poff + idx] = q->sort_by != 0 ? key[k] : (uint64_t)aux[k];
-                }
-                ++idx;
+                /* b* is recomputed whenever the stored count crosses a multiple of 256 */
+                const uint32_t after = idx + 1;
+                crossed = (idx >> 8) != (after >> 8) && may_raise_bstar(p, q, after);
+            } else if (idx < st->pool_cap) {
+                /* second pass: every match at or above the exact b* goes to the query's slice of the pool */
+                const size_t o = (size_t)st->pool_off + idx;
+                p.pool_w[o] = w; p.pool_d[o] = d; p.pool_k[o] = kv;
             }
         }
     }
-    /* raise b* whenever the stored count crosses a multiple of 256 (and topk matches exist) */
-    const uint32_t after = base + nkeep;
-    /* (not before half of what the top-k kernel can rank is in use: small match sets stay unpruned, so
-     * their known_matching_docs is reproduced exactly) */
-    if (p.pass == 0 && (base >> 8) != (after >> 8) && after >= q->topk && after >= p.keep_cap / 2)
-        raise_bstar_warp(q, st, hist, lane);
-}
-
-/* count_only: matches already proven unable to reach the top-k (MaxScore bound below b*): they are
- * counted in the exact match total but neither scored nor stored */
-__device__ __forceinline__ void emit_matches(const XgmKernelParams& p, const XgmDevQuery* q, uint32_t qi, uint32_t lane,
-                                             uint32_t alive, const double acc[4], const uint32_t c[4],
-                                             const uint32_t aux[4], uint32_t count_only = 0) {
-    if (!__any_sync(FULL, alive != 0)) return;
-    emit_matches_impl(p, q, qi, lane, alive, acc[0], acc[1], acc[2], acc[3], c[0], c[1], c[2], c[3], aux[0], aux[1],
-                      aux[2], aux[3], count_only);
+    uint32_t m = __ballot_sync(FULL, crossed);
+    while (m) {
+        const uint32_t l = (uint32_t)__ffs(m) - 1u;
+        m &= m - 1u;
+        const uint32_t rq = __shfl_sync(FULL, qi, l);
+        raise_bstar_warp(&p.queries[rq], &p.qstate[rq], p.hist + (size_t)rq * XGM_NBINS, lane);
+    }
 }
 
 /* ------------------------------------------------------------------ shared per-warp scratch */
@@ -825,7 +793,9 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(const __gr
                     }
                 }
             }
-            emit_matches(p, q, wi.query, lane, alive, acc, c, aux);
+            count_matches(p, wi.query, __popc(alive), lane);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) emit_match_lanes(p, lane, alive >> k & 1u, wi.query, acc[k], c[k], aux[k], false);
             dh = nh;
             buf ^= 1u;
         }
@@ -866,58 +836,6 @@ static_assert(XGM_BM_RUN <= 16, "q1src keeps a query slot in 4 bits");
 /* 4.6 KB per warp, 37 KB per CTA: with 4 CTAs per SM the shared-memory carve-out stays at 164 KB and the
  * bitmap probes keep ~90 KB of L1 (51 KB per CTA would push the carve-out to 228 KB and leave the probes
  * almost no L1). */
-
-/* Per-lane emission of one match (lanes of a flush belong to different queries): count it, keep it unless
- * its bucket is already below the query's pruning bucket.  Warp-converged call. */
-__device__ __forceinline__ void emit_match_lanes(const XgmKernelParams& p, uint32_t lane, bool alive, uint32_t qi, double w,
-                                                 uint32_t d, uint32_t aux, bool count = true) {
-    bool crossed = false;
-    /* A query with 10^5..10^6 matches would otherwise send every one of them to the same two words (total, maxw):
-     * same-address atomics serialise in L2 and one such query doubled the launch time of a 4096-query batch.  The
-     * lanes of one query are counted by their lowest lane, and maxw — which only rises — is read first. */
-    if (p.pass == 0 && count) {
-        const uint32_t grp = __match_any_sync(FULL, alive ? qi : 0xffffffffu);
-        if (alive && lane == (uint32_t)__ffs(grp) - 1u) atomicAdd(&p.qstate[qi].total, (uint32_t)__popc(grp));
-    }
-    if (alive) {
-        const XgmDevQuery* q = &p.queries[qi];
-        XgmQState* st = &p.qstate[qi];
-        if (p.pass == 0) {
-            const unsigned long long wb = (unsigned long long)__double_as_longlong(w);
-            if (wb >= *reinterpret_cast<volatile unsigned long long*>(&st->maxw)) {
-                const unsigned long long oldmax = atomicMax(&st->maxw, wb);
-                if (q->log_raises && wb >= oldmax) log_raise(p, qi, wb, d, aux);
-            }
-        }
-        const uint64_t key = q->sort_by != 0 ? doc_sort_key(p, q, d) : 0ull;
-        const uint32_t bkt = match_bucket(q, w, key);
-        if (bkt >= live_bstar(st) && q->topk != 0) {
-            const uint32_t idx = atomicAdd(&st->stored, 1u);
-            const uint64_t kv = q->sort_by != 0 ? key : (uint64_t)aux;
-            if (p.pass == 0) {
-                atomicAdd(p.hist + (size_t)qi * XGM_NBINS + bkt, 1u);
-                if (idx < p.match_cap) {
-                    const size_t o = (size_t)qi * p.match_cap + idx;
-                    p.match_w[o] = w; p.match_d[o] = d; p.match_k[o] = kv;
-                }
-                const uint32_t after = idx + 1;
-                /* (AND: not before half of what the top-k kernel can rank is in use, so that small match sets stay
-                 * unpruned and their known_matching_docs is exact; an OR's union is far larger than that anyway) */
-                crossed = (idx >> 8) != (after >> 8) && after >= q->topk && (q->route == XGM_ROUTE_OR || after >= p.keep_cap / 2);
-            } else if (idx < st->pool_cap) {
-                const size_t o = (size_t)st->pool_off + idx;
-                p.pool_w[o] = w; p.pool_d[o] = d; p.pool_k[o] = kv;
-            }
-        }
-    }
-    uint32_t m = __ballot_sync(FULL, crossed);
-    while (m) {
-        const uint32_t l = (uint32_t)__ffs(m) - 1u;
-        m &= m - 1u;
-        const uint32_t rq = __shfl_sync(FULL, qi, l);
-        raise_bstar_warp(&p.queries[rq], &p.qstate[rq], p.hist + (size_t)rq * XGM_NBINS, lane);
-    }
-}
 
 /* One flat loop with five states, so that each piece of code exists once and nothing is called from the hot
  * path: score 32 matches (stage 2 full, or out of work) → finish 32 candidates (stage 1 full, or the item
@@ -1336,7 +1254,11 @@ __global__ void __launch_bounds__(OR_WARPS * 32) xgm_or_kernel(const __grid_cons
                     aux[k] = __popc(present[k]);
                 }
             }
-            emit_matches(p, q, wi.query, lane, owned, acc, c, aux, skip);
+            /* the documents MaxScore skipped are matches too: counted, never scored or stored */
+            count_matches(p, wi.query, __popc(owned), lane);
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                emit_match_lanes(p, lane, (owned & ~skip) >> k & 1u, wi.query, acc[k], c[k], aux[k], false);
             __syncwarp();
         }
     }
@@ -1465,8 +1387,7 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, 3) xgm_or3_kernel(const __grid
         /* ---- next work item ---- */
         if (db >= it_b1) {
             if (total_acc || it_b1) { /* close the previous item: its owned documents are matches */
-                const uint32_t t = __reduce_add_sync(FULL, total_acc);
-                if (lane == 0 && t && p.pass == 0) atomicAdd(&p.qstate[it_query].total, t);
+                count_matches(p, it_query, total_acc, lane);
                 total_acc = 0; it_b1 = 0; db = 0;
             }
             uint32_t item;
@@ -1570,10 +1491,7 @@ __global__ void __launch_bounds__(OR3_WARPS * 32, 3) xgm_or3_kernel(const __grid
             ++db;
         }
     }
-    if (total_acc || it_b1) {
-        const uint32_t t = __reduce_add_sync(FULL, total_acc);
-        if (lane == 0 && t && p.pass == 0) atomicAdd(&p.qstate[it_query].total, t);
-    }
+    if (total_acc || it_b1) count_matches(p, it_query, total_acc, lane);
 }
 
 cudaError_t xgm_launch_or3(const XgmKernelParams& p, int grid, int phase, cudaStream_t s) {
@@ -1705,8 +1623,7 @@ __global__ void __launch_bounds__(TILE_WARPS * 32, 4) xgm_or_tile_kernel(const _
 #pragma unroll
             for (int j = 0; j < OR3_MAX_LEAVES; ++j) w[j] = wn[j];
         }
-        const uint32_t t = __reduce_add_sync(FULL, total_acc);
-        if (lane == 0 && t && p.pass == 0) atomicAdd(&p.qstate[qi].total, t);
+        count_matches(p, qi, total_acc, lane);
     }
     __syncwarp();
     if (qn) flush(qn);
@@ -1799,30 +1716,6 @@ __device__ __forceinline__ void bitonic_sort_candidates(double* sw, uint64_t* sk
             }
             __syncthreads();
         }
-    }
-}
-
-/* Highest bin b with at least `want` entries in bins [b, XGM_NBINS) of a shared-memory histogram (0 if the
- * whole histogram holds fewer), found by warp 0: 32 bins per lane, a suffix scan over the lanes, then a
- * walk inside the one lane's bins.  Result in *out (shared); the caller synchronises. */
-__device__ __forceinline__ void threshold_bin(const uint32_t* lh, uint32_t want, uint32_t tid, uint32_t* out) {
-    if (tid >= 32) return;
-    const uint32_t per = XGM_NBINS / 32;
-    uint32_t sum = 0;
-    for (uint32_t i = 0; i < per; ++i) sum += lh[tid * per + i];
-    uint32_t suffix = sum; /* entries in the bins of lanes >= tid */
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_down_sync(FULL, suffix, o);
-        if ((int)tid + o < 32) suffix += t;
-    }
-    const uint32_t ok = __ballot_sync(FULL, suffix >= want);
-    if (ok == 0) { if (tid == 0) *out = 0; return; }
-    const uint32_t lane = 31u - (uint32_t)__clz(ok); /* highest lane whose suffix reaches `want` */
-    if (tid == lane) {
-        uint32_t cum = suffix - sum, b = (tid + 1) * per;
-        while (b > tid * per && cum < want) { --b; cum += lh[b]; }
-        *out = b;
     }
 }
 
@@ -1988,7 +1881,10 @@ __device__ __forceinline__ void topk_one_query(const XgmKernelParams& p, const u
         __syncthreads();
         for (uint32_t i = tid; i < n; i += TOPK_THREADS) atomicAdd(&lh[match_bucket(q, sw[i], sk[i])], 1u);
         __syncthreads();
-        threshold_bin(lh, topk, tid, &s_prefix[0]);
+        if (tid < 32) {
+            const uint32_t b = bin_of_rank(lh, topk, tid);
+            if (tid == 0) s_prefix[0] = b;
+        }
         if (tid == 32) s_n = 0;
         __syncthreads();
         const uint32_t bsel = s_prefix[0];
