@@ -247,7 +247,12 @@ typedef struct xgm_mset_info {
  * match sets that were pruned on the device, or a check_at_least in between (where the reference's
  * min_weight lags, protomset.h:377-398), the lower bound / estimate are conservative (still valid
  * bounds) and this flag is set.  Docids, weights, max_possible,
- * max_attained, the upper bound and exact_matches are always exact. */
+ * max_attained, percent_scale_factor, the upper bound and exact_matches are always exact.
+ * percent_scale_factor needs the number of subqueries matching the FIRST document in docid order that attains
+ * max_attained (ProtoMSet::update_max_weight, protomset.h:174-183).  Where that document need not be among the
+ * results (an OR or OP_AND_MAYBE sorted by value), the kernels keep a record of the matches that reach the running
+ * best weight; a query with more such matches than that record holds (XGM_RAISE_LOG, e.g. a tie of more than 64
+ * matches at the best weight) is declined with XGM_E_UNIMPLEMENTED, never answered with a guessed percentage. */
 #define XGM_MSET_BOUNDS_APPROX 1u
 /* OR queries only: MaxScore skipped whole posting-list segments that cannot reach the top-k (what
  * OrPostList's w_min pruning does in the reference, orpostlist.cc:113-155), so exact_matches counts only

@@ -95,6 +95,7 @@ def lib():
         L.orc_index_load_flat.argtypes = [C.c_char_p]
         L.orc_index_free.argtypes = [C.POINTER(_Index)]
         L.orc_index_make_sparse.argtypes = [C.POINTER(_Index), C.c_uint32, C.c_uint32]
+        L.orc_index_set_slot0.argtypes = [C.POINTER(_Index), C.c_void_p, C.c_void_p]
         L.orc_query_defaults.argtypes = [C.POINTER(_Query)]
         L.orc_match.argtypes = [C.POINTER(_Index), C.POINTER(_Query), C.POINTER(_MSet)]
         L.orc_merge.argtypes = [C.POINTER(_MSet), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_int,
@@ -194,6 +195,14 @@ class Index:
     def make_sparse(self, mod0: int, mod1: int):
         """Drop slot values by the rule of `ref_runner build --mvalues-sparse mod0 mod1`."""
         lib().orc_index_make_sparse(self._p, mod0, mod1)
+
+    def set_slot0(self, nvals: np.ndarray, vals: np.ndarray):
+        """Slot-0 values of a hand-made corpus: nvals[lastdocid + 1] (0..3 each), vals[lastdocid + 1, 3]."""
+        n = self.lastdocid + 1
+        nv = np.ascontiguousarray(nvals, np.uint8)
+        v = np.ascontiguousarray(vals, np.uint64)
+        assert nv.shape == (n,) and v.shape == (n, 3)
+        lib().orc_index_set_slot0(self._p, nv.ctypes.data_as(C.c_void_p), v.ctypes.data_as(C.c_void_p))
 
     def close(self):
         if self._p:

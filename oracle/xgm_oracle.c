@@ -500,6 +500,18 @@ void orc_index_make_sparse(orc_index* ix, uint32_t mod0, uint32_t mod1) {
     }
 }
 
+void orc_index_set_slot0(orc_index* ix, const uint8_t* nvals, const uint64_t* vals) {
+    if (!ix) return;
+    const size_t n = (size_t)ix->lastdocid + 1;
+    if (!ix->nvals0) {
+        ix->nvals0 = (uint8_t*)xcalloc(n, 1);
+        ix->vals0 = (uint64_t*)xcalloc(3 * n, 8);
+        ix->val1 = (uint64_t*)xcalloc(n, 8);
+    }
+    memcpy(ix->nvals0, nvals, n);
+    memcpy(ix->vals0, vals, 3 * n * 8);
+}
+
 /* (termfreq min, max, est, max weight) of a subtree, as the reference's PostList classes report them */
 typedef struct { uint32_t mn, mx, est; double maxw; } node_t;
 

@@ -115,6 +115,9 @@ void orc_index_free(orc_index*);
 /* Drop slot-0 values of documents whose smallest value is a multiple of mod0 and slot-1 values that are
  * multiples of mod1 (0 = keep all) — the rule of `ref_runner build --mvalues-sparse`. */
 void orc_index_make_sparse(orc_index*, uint32_t mod0, uint32_t mod1);
+/* Give slot 0 the values of a hand-made corpus (an XGMFLAT1 file carries none): nvals[lastdocid + 1] values per
+ * document (0..3), vals[3 * (lastdocid + 1)] ascending per document.  Both are copied. */
+void orc_index_set_slot0(orc_index*, const uint8_t* nvals, const uint64_t* vals);
 int orc_term_lookup(const orc_index*, const char* name, uint32_t* id);
 
 void orc_query_defaults(orc_query* q);

@@ -11,7 +11,7 @@ import pytest
 
 from oracle import oracle as O
 from tests.flatfile import write_flat
-from tests.util import assert_mset_equal
+from tests.util import assert_mset_equal, bits
 from xapiand_b200 import xgm
 
 pytestmark = pytest.mark.gpu
@@ -117,6 +117,17 @@ def test_degenerate_arguments(edge):
             assert m.matches_lower_bound <= ref.lb and m.matches_upper_bound == ref.ub, c
         else:
             assert (m.matches_lower_bound, m.matches_estimated_raw, m.matches_upper_bound) == (ref.lb, ref.est, ref.ub), c
+    # an OR whose `first` is past every match keeps no results but still has the percentage scale of its best
+    # document, whose number of matching leaves varies per document
+    for c in (dict(first=100000, maxitems=10, check_at_least=0), dict(first=100000, maxitems=10, check_at_least=50),
+              dict(first=7000, maxitems=0, check_at_least=7000)):
+        m = s.search([xgm.Query(xgm.OP_OR, [names[t], names[u], "k_rare"], **c)])[0]
+        ref = orc.match(O.Query(op=O.OP_OR, terms=[t, u, names.index("k_rare")], **c))
+        assert m.status == 0 and m.size() == 0 and len(ref.docids) == 0, c
+        assert ref.percent_scale_factor > 0, c
+        assert (m.matches_lower_bound, m.matches_estimated_raw, m.matches_upper_bound) == (ref.lb, ref.est, ref.ub), c
+        assert bits(m.percent_scale_factor) == bits(ref.percent_scale_factor), c
+        assert bits(m.max_attained) == bits(ref.max_attained), c
     # OR with an absent leaf behaves like the OR of the others; AND with an absent leaf is empty
     m = s.search([xgm.Query(xgm.OP_AND, [names[t], "zzz_absent"], maxitems=10)])[0]
     assert m.size() == 0 and m.status == 0

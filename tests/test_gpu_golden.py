@@ -284,8 +284,7 @@ def test_cuda_matches_reference_more_regimes(tag):
         assert m.matches_upper_bound == q["ub"], ctx
         if not (m.flags & 1):
             assert (m.matches_lower_bound, m.get_matches_estimated()) == (q["lb"], q["est"]), ctx
-        if not (q["op"] == "OR" and q.get("sort")):  # OR + value sort: percent scale is a documented approximation
-            assert [O.convert_to_percent(w, m.percent_scale_factor) for w in m.weights] == q["percents"], ctx
+        assert [O.convert_to_percent(w, m.percent_scale_factor) for w in m.weights] == q["percents"], ctx
     assert declined < len(keep) // 4
 
 

@@ -24,7 +24,7 @@ def gen_queries(rng: random.Random, n, topranks, ndocs, ops=("AND",), ks=(3,), m
 def assert_matches_oracle(got, ref, ctx=""):
     """assert_mset_equal, except that what an approximation flag licenses is checked in its weaker form:
     with BOUNDS_APPROX (1) lb <= ref.lb and lb <= est <= ub; with COUNT_LOWER_BOUND (2) exact <= ref.exact.
-    The upper bound is always exact."""
+    The upper bound and the percentage scale are always exact."""
     approx = bool(got.flags & 1)
     assert_mset_equal(got, ref, ctx, check_counts=not approx)
     assert got.matches_upper_bound == ref.ub, f"{ctx}: ub {got.matches_upper_bound} vs {ref.ub}"
@@ -46,8 +46,10 @@ def assert_mset_equal(got, ref, ctx="", check_counts=True):
     assert gw.tobytes() == rw.tobytes(), f"{ctx}: weights differ (max rel {np.max(np.abs(gw-rw)/np.maximum(rw,1e-300)) if len(gw) else 0})"
     assert bits(got.max_possible) == bits(ref.max_possible), f"{ctx}: max_possible {got.max_possible} vs {ref.max_possible}"
     assert bits(got.max_attained) == bits(ref.max_attained), f"{ctx}: max_attained {got.max_attained} vs {ref.max_attained}"
+    # no flag makes the percentage scale approximate (include/xgm.h)
+    assert bits(got.percent_scale_factor) == bits(ref.percent_scale_factor), \
+        f"{ctx}: percent scale {got.percent_scale_factor!r} vs {ref.percent_scale_factor!r}"
     if check_counts:
         assert (got.matches_lower_bound, got.matches_estimated_raw, got.matches_upper_bound) == (ref.lb, ref.est, ref.ub), \
             f"{ctx}: bounds {(got.matches_lower_bound, got.matches_estimated_raw, got.matches_upper_bound)} vs {(ref.lb, ref.est, ref.ub)}"
         assert got.exact_matches == ref.exact, f"{ctx}: exact {got.exact_matches} vs {ref.exact}"
-        assert bits(got.percent_scale_factor) == bits(ref.percent_scale_factor), f"{ctx}: percent scale"

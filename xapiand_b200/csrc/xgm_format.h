@@ -119,9 +119,11 @@ struct XgmQState {
 /* ProtoMSet::update_max_weight (matcher/protomset.h:174-183) remembers how many subqueries matched the
  * best-weighted document — the numerator of percent_scale_factor.  When that number varies per document (OR,
  * AND_MAYBE) and the MSet is NOT ordered by weight, the best-weighted document need not be among the results,
- * so queries that ask for it (XgmDevQuery::log_raises) log every match that attains the running maximum:
- * {weight bits, docid, matching subqueries}.  The running maximum only rises, so the log stays short
- * (~ln(matches) entries); a query whose log overflows is declined. */
+ * so queries that ask for it (XgmDevQuery::log_raises) log every match that attains the
+ * running maximum: {weight bits, docid, matching subqueries}.  The running maximum only rises, so with distinct
+ * weights the log holds about ln(matches) entries; but every match that ties the running maximum is logged too,
+ * so a tie of more than XGM_RAISE_LOG matches at the best weight (or at a running maximum reached before it)
+ * overflows it, and a query whose log overflows is declined. */
 #define XGM_RAISE_LOG 64u
 struct XgmRaise { unsigned long long wbits; uint32_t docid, subqs; };
 

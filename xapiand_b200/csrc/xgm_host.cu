@@ -1655,11 +1655,18 @@ static void plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, Planned
     pq.alg_bytes += 16ull * pq.topk;
 
     /* `first` at or beyond the largest possible match count: ProtoMSet never fills (protomset.h:497-505),
-     * the MSet is empty and all three bounds equal the exact match count — count on the device only */
-    if (pq.first >= pq.tf_max && cal != 0) { pq.count_only = true; dq.topk = 0; }
-    else if (pq.topk > s->max_topk) { pq.status = XGM_E_INVALID; return; }
+     * the MSet is empty and all three bounds equal the exact match count — count on the device only.  Where the
+     * number of matching subqueries varies per document, percent_scale_factor still needs that of the first
+     * best-weighted document (ProtoMSet saw every match): keep that one document, in relevance order — nothing is
+     * returned, so the order asked for does not matter — and read its count as for any relevance-ordered query. */
+    if (pq.first >= pq.tf_max && cal != 0) {
+        pq.count_only = true;
+        const bool varies = dq.route == XGM_ROUTE_OR || pq.aux_subqs;
+        dq.topk = varies ? 1u : 0u;
+        if (varies) dq.sort_by = XGM_SORT_REL;
+    } else if (pq.topk > s->max_topk) { pq.status = XGM_E_INVALID; return; }
     /* pruning buckets: linear in the primary sort key (weight, or the sort value for VAL sorts) */
-    if (q.sort_by == XGM_SORT_REL || q.sort_by == XGM_SORT_REL_VAL) {
+    if (dq.sort_by == XGM_SORT_REL || dq.sort_by == XGM_SORT_REL_VAL) {
         dq.bucket_scale = pq.bucket_max > 0 ? (double)XGM_NBINS / pq.bucket_max : 0.0;
     } else {
         dq.bucket_key_min = ix->slot_min[q.sort_slot];
@@ -1668,7 +1675,7 @@ static void plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, Planned
 
     /* percent_scale_factor needs the number of subqueries matching the best-WEIGHTED document: when that varies
      * per document and the order is not by weight alone, have the kernels log the running-maximum matches */
-    dq.log_raises = (dq.route == XGM_ROUTE_OR || pq.aux_subqs) && q.sort_by != XGM_SORT_REL ? 1u : 0u;
+    dq.log_raises = (dq.route == XGM_ROUTE_OR || pq.aux_subqs) && dq.sort_by != XGM_SORT_REL ? 1u : 0u;
     pq.log_raises = dq.log_raises != 0;
     if (cal == 0) return; /* bounds only, matcher.cc:437-461 */
     /* a list every match is in is absent (an AND's terms, the FILTER terms on either base): the MSet is empty */
@@ -2037,7 +2044,8 @@ static void finish_info(const PlannedQuery& pq, const XgmDevResult* dr, const ui
         if (pq.check_at_least > pq.topk + 1 && known < dr->exact && !pq.count_only && pq.sort_by == XGM_SORT_REL_VAL)
             o->flags |= XGM_MSET_BOUNDS_APPROX; /* relevance-then-value still uses the simple counting rule */
         if (dr->flags & (XGM_RES_LOST | XGM_RES_PENDING)) o->status = XGM_E_UNIMPLEMENTED; /* lost or pending: pathological tie mass */
-        if (dr->flags & XGM_RES_APPROX) o->flags |= XGM_MSET_BOUNDS_APPROX;
+        /* a count-only query keeps one document only for the percentage scale: its bounds are the exact count */
+        if ((dr->flags & XGM_RES_APPROX) && !pq.count_only) o->flags |= XGM_MSET_BOUNDS_APPROX;
         if (dr->flags & XGM_RES_SKIPPED) o->flags |= XGM_MSET_BOUNDS_APPROX | XGM_MSET_COUNT_LOWER_BOUND;
         /* with a value-range source in the AND the reference's lower bound / estimate also fold in
          * ValueRangePostList::get_termfreq_est (valuerangepostlist.cc:70-130), which is not restated */
@@ -2052,9 +2060,10 @@ static void finish_info(const PlannedQuery& pq, const XgmDevResult* dr, const ui
     o->n = size > pq.first ? size - pq.first : 0;
     if ((size != 0 || (pq.count_only && pq.on_device && dr->exact != 0)) && max_w != 0.0) {
         /* ProtoMSet::finalise_percentages protomset.h:466-471: AND → every subquery matched */
-        /* AND: every leaf matches; OR sorted by relevance: leaves matching the best document */
+        /* AND: every leaf matches; OR ranked by relevance on the device (count-only queries included): leaves
+         * matching the first ranked document */
         uint32_t subqs = dr->max_subqs;
-        if (is_or && pq.sort_by == XGM_SORT_REL && keys) subqs = (uint32_t)keys[0];
+        if (is_or && (pq.sort_by == XGM_SORT_REL || pq.count_only) && keys) subqs = (uint32_t)keys[0];
         if (pq.log_raises) {
             /* ProtoMSet::update_max_weight: the FIRST document in docid order that attains the maximum */
             if (!raises || nraise > XGM_RAISE_LOG) { o->status = XGM_E_UNIMPLEMENTED; return; }
