@@ -377,9 +377,11 @@ def have_reference() -> bool:
 
 
 def ref_build(out_dir: str, ndocs: int, vocab: int, seed: int = 12345, nshards: int = 1, shard: int = 0,
-              values: bool = False, env=None, mvalues: bool = False, sparse=None) -> dict:
+              values: bool = False, env=None, mvalues: bool = False, sparse=None, boolean_terms: int = 0) -> dict:
     cmd = [REF_RUNNER, "build", "--out", out_dir, "--docs", str(ndocs), "--vocab", str(vocab),
            "--seed", str(seed), "--nshards", str(nshards), "--shard", str(shard)]
+    if boolean_terms:  # XB0.. as Document::add_boolean_term (wdf 0); see oracle/ref_runner.cc
+        cmd += ["--boolean-terms", str(boolean_terms)]
     if values:
         cmd.append("--values")
     if mvalues:  # Xapiand's slot encoding: StringList of Serialise::positive keys

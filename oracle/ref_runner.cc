@@ -6,7 +6,7 @@
  * bench.py.  The product never links or executes this.
  *
  *   ref_runner build  --out DIR --docs N --vocab V --seed S [--nshards n --shard s] [--values | --mvalues]
- *                     [--termlist] [--range-first a --range-last b]
+ *                     [--termlist] [--range-first a --range-last b] [--boolean-terms K]
  *                                                       write a glass DB through WritableDatabase
  *                                                       (--range-*: only global docids a..b, as local 1..)
  *                                                       --mvalues: value slots the way Xapiand writes them —
@@ -100,6 +100,7 @@ static int cmd_build(const Args& a) {
     uint32_t shard = (uint32_t)strtoul(a.get("--shard", "0").c_str(), nullptr, 10);
     bool values = a.flag("--values");
     bool mvalues = a.flag("--mvalues");
+    const uint32_t nbool = (uint32_t)strtoul(a.get("--boolean-terms", "0").c_str(), nullptr, 10);
     /* --mvalues-sparse m0 m1: no slot-0 value where the smallest value is a multiple of m0, no slot-1 value
      * where it is a multiple of m1 (documents without a value: SerialiseKey's MAX/MIN_STR_CMPVALUE path) */
     uint32_t sp0 = 0, sp1 = 0;
@@ -129,6 +130,11 @@ static int cmd_build(const Args& a) {
         uint32_t len = xgm_corpus_doc(&z, seed, d, ranks);
         uint32_t n = xgm_corpus_collapse(ranks, len, wdf);
         Xapian::Document doc;
+        /* --boolean-terms K: Document::add_boolean_term (wdf 0, no length), the way Xapiand stores boolean fields:
+         * XBj on the docids that are multiples of j + 2; the multiples of 50 hold nothing else (length 0) */
+        for (uint32_t j = 0; j < nbool; ++j)
+            if (d % (j + 2) == 0) doc.add_boolean_term("XB" + std::to_string(j));
+        if (nbool && d % 50 == 0) n = 0;
         for (uint32_t i = 0; i < n; ++i) doc.add_term(names[ranks[i]], wdf[i]);
         if (values) {
             uint64_t v0[3], v1;

@@ -831,6 +831,9 @@ int orc_match(const orc_index* ix, const orc_query* qin, orc_mset* out) {
                 for (uint32_t i = 0; i < n; ++i) {
                     uint32_t j = order[i];
                     if (q->filter_weighted && src_pos == i) weight += src_w; /* ExternalPostList::get_weight */
+                    /* LeafPostList::get_weight api/leafpostlist.cc:57-63: 0 for a leaf without a Weight, which
+                     * get_sumpart is never asked about (at wdf 0 it would be 0 * (0 / 0)) */
+                    if (q->factors && q->factors[j] == 0.0) continue;
                     weight += orc_bm25_sumpart(tw[j], len_factor, q->k1, q->b, q->min_normlen, wl[j][pos[j]], doclen);
                 }
                 if (q->filter_weighted && src_pos == n) weight += src_w;
@@ -852,9 +855,12 @@ int orc_match(const orc_index* ix, const orc_query* qin, orc_mset* out) {
                     if (prog[i] >= 0) {
                         uint32_t j = (uint32_t)prog[i];
                         if (pos[j] < len[j] && dl[j][pos[j]] == did) {
-                            stk[sp] = orc_bm25_sumpart(tw[j], len_factor, q->k1, q->b, q->min_normlen, wl[j][pos[j]], doclen);
+                            const int weighted = !q->factors || q->factors[j] != 0.0;
+                            /* LeafPostList::get_weight: 0 without a Weight */
+                            stk[sp] = weighted ? orc_bm25_sumpart(tw[j], len_factor, q->k1, q->b, q->min_normlen,
+                                                                  wl[j][pos[j]], doclen) : 0.0;
                             stkp[sp] = 1;
-                            if (!q->factors || q->factors[j] != 0.0) ++subqs;
+                            if (weighted) ++subqs;
                         } else { stk[sp] = 0; stkp[sp] = 0; }
                         ++sp;
                     } else {

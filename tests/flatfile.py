@@ -5,13 +5,14 @@ import struct
 import numpy as np
 
 
-def write_flat(path, doclen, terms, wdf_ub_db=None):
+def write_flat(path, doclen, terms, wdf_ub_db=None, doccount=None):
     """doclen: array indexed by docid (entry 0 unused, 0 = unused docid).
-    terms: list of (name, docids, wdfs), names ascending (like Database::allterms_begin)."""
+    terms: list of (name, docids, wdfs), names ascending (like Database::allterms_begin).
+    doccount: the number of documents, where some have length 0 (only boolean terms)."""
     doclen = np.asarray(doclen, np.uint32)
     lastdocid = len(doclen) - 1
     used = doclen[1:][doclen[1:] > 0]
-    doccount = int(len(used))
+    doccount = int(len(used)) if doccount is None else int(doccount)
     total = int(doclen.sum())
     lb = int(used.min()) if doccount else 0
     ub = int(used.max()) if doccount else 0

@@ -1,8 +1,8 @@
 """Range-major bitmap ANDs whose queries share their driver list (the rarest required term): the planner packs up to
-3 of them into a run, and the AND kernel decodes the run's driver blocks once per range and probes them for every
-query of the run.  A driver with far more queries than a run holds, runs of 1, 2 and 3 queries, term groups and
-value ranges mixed inside runs, and tie masses that take the second matching pass while the other queries of their run
-do not are compared with the oracle."""
+XGM_BM_RUN (6) of them into a run, and the AND kernel decodes the run's driver blocks once per range and probes them
+for every query of the run.  A driver with far more queries than a run holds, runs of 1, 2 and 6 queries, term groups
+and value ranges mixed inside runs, and tie masses that take the second matching pass while the other queries of their
+run do not are compared with the oracle."""
 import random
 
 import pytest
@@ -12,7 +12,7 @@ from xapiand_b200 import xgm
 
 pytestmark = pytest.mark.gpu
 
-RUN = 3  # queries per run (XGM_BM_RUN)
+RUN = 6  # queries per run (XGM_BM_RUN)
 PROBES = range(30)  # more frequent than every driver below, so that the driver stays the rarest required term
 
 
@@ -54,7 +54,7 @@ def tie_run(rng):
 @pytest.mark.parametrize("bpi", [None, 1, 32])
 @pytest.mark.parametrize("range_bits", [8, 14, 17])
 def test_driver_runs(corpus, monkeypatch, range_bits, bpi):
-    """40 ANDs led by one driver (14 runs), runs of 3, 2 and 1 queries, 12 ANDs with mixed tests led by one driver
+    """40 ANDs led by one driver (7 runs), runs of 6, 2 and 1 queries, 12 ANDs with mixed tests led by one driver
     and two runs that hold two tie masses, among 250 other all-bitmap ANDs, at 118, 2 and 1 document ranges over
     the 30k docids and the default, 1 and 32 driver blocks per item (32: the widest block field of a queued
     candidate)."""

@@ -88,6 +88,9 @@ struct XgmDevQuery {
     uint32_t or_nreq;                   /* OR under OP_FILTER: terms[nterms .. nterms+or_nreq) must hold the document, then nnot excluded ones */
     uint32_t log_raises;                /* record the matches that attain the running maximum weight (XGM_RAISE_LOG) */
     uint32_t probe_coarse;              /* bitmap AND: test terms[1]'s coarse bit before its fine bit (sparse terms[1]) */
+    uint32_t unweighted;                /* AND: bit j set = required list j has no Weight (an OP_FILTER boolean term or a
+                                           factor-0 leaf) and adds nothing, as LeafPostList::get_weight returns 0 without
+                                           one: its BM25 sumpart is not computed (at wdf 0 it would be 0 * (0 / 0)) */
     XgmDevTerm terms[XGM_DEV_MAX_TERMS]; /* AND: ascending termfreq (MultiAndPostList order) */
 };
 

@@ -1445,8 +1445,8 @@ static xgm_status weigh_terms(const xgm_index* ix, const xgm_query& q, PlanTerms
     return XGM_OK;
 }
 
-/* Device slot of leaf `id` (0xffffffffu: not in this index) with its weight pair.  A boolean leaf has (0.0, 0.0):
- * it adds +0.0 to the weight sum, which leaves the sum unchanged. */
+/* Device slot of leaf `id` (0xffffffffu: not in this index) with its weight pair.  A boolean leaf has (0.0, 0.0); the
+ * AND kernels skip it altogether (XgmDevQuery::unweighted). */
 static void put_term(const xgm_index* ix, XgmDevTerm& d, uint32_t id, double termweight, double maxpart) {
     d.termweight = termweight;
     d.maxpart = maxpart;
@@ -1561,6 +1561,7 @@ static void plan_and_route(const xgm_index* ix, const xgm_query& q, const PlanTe
         const bool base = fi >= t.nfilter || (bi < n && t.ltf[order[bi]] <= fin[fi].tf);
         const uint32_t j = base ? order[bi++] : fin[fi++].idx;
         if (slot == 1) tf1 = t.ltf[j];
+        if (!base || (q.factors && q.factors[j] == 0.0)) dq.unweighted |= 1u << slot;
         put_term(ix, dq.terms[slot++], t.ids[j], base ? t.tw[j] : 0.0, base ? t.maxpart[j] : 0.0);
     }
     /* The bitmap AND kernel probes terms[1] for every driver posting.  Where a coarse bit (8 docids) is rarely set,

@@ -703,7 +703,7 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(const __gr
                     if (alive >> k & 1u) {
                         uint32_t tf = tb ? unpack_sm(ws.stage, 4 * lane + k, tb, tmask) : 0u;
                         dl[k] = __ldg(&p.doclen[c[k]]);
-                        acc[k] = bm25_sumpart(tw0, q, tf, dl[k]);
+                        acc[k] = (q->unweighted & 1u) ? 0.0 : bm25_sumpart(tw0, q, tf, dl[k]);
                         if (q->src_pos == 0) acc[k] = __dadd_rn(q->src_weight, acc[k]);
                         else if (q->src_pos == 1) acc[k] = __dadd_rn(acc[k], q->src_weight);
                     }
@@ -719,14 +719,19 @@ __global__ void __launch_bounds__(MATCH_WARPS * 32, 3) xgm_and_kernel(const __gr
                     if (j == 1) {
                         /* first confirmation: fetch doclen and the driver's own wdf lazily */
                         dl[k] = __ldg(&p.doclen[c[k]]);
-                        uint32_t tf0 = unpack_gl(p.tfs, dh.tf_off, 4 * lane + k, XGM_HDR_TF_BITS(dh.meta));
-                        acc[k] = bm25_sumpart(tw0, q, tf0, dl[k]);
+                        acc[k] = 0.0;
+                        if (!(q->unweighted & 1u)) {
+                            uint32_t tf0 = unpack_gl(p.tfs, dh.tf_off, 4 * lane + k, XGM_HDR_TF_BITS(dh.meta));
+                            acc[k] = bm25_sumpart(tw0, q, tf0, dl[k]);
+                        }
                         if (q->src_pos == 0) acc[k] = __dadd_rn(q->src_weight, acc[k]);
                     }
                     if (q->src_pos == j) acc[k] = __dadd_rn(acc[k], q->src_weight);
-                    uint32_t tfj = unpack_gl(p.tfs, bh.tf_off, pos, XGM_HDR_TF_BITS(bh.meta));
                     /* MultiAndPostList::get_weight: result += plist[i]->get_weight(), in plist order */
-                    acc[k] = __dadd_rn(acc[k], bm25_sumpart(twj, q, tfj, dl[k]));
+                    if (!(q->unweighted >> j & 1u)) {
+                        uint32_t tfj = unpack_gl(p.tfs, bh.tf_off, pos, XGM_HDR_TF_BITS(bh.meta));
+                        acc[k] = __dadd_rn(acc[k], bm25_sumpart(twj, q, tfj, dl[k]));
+                    }
                     if (j + 1 == nterms && q->src_pos == nterms) acc[k] = __dadd_rn(acc[k], q->src_weight);
                 };
                 const uint64_t bm_off = q->terms[j].bm_off;
@@ -895,13 +900,15 @@ __global__ void __launch_bounds__(BM3_WARPS * 32, 4) xgm_and_bm3_kernel(const __
                 const XgmDevQuery* mq = &p.queries[qi];
                 const uint32_t dlen = __ldg(&p.doclen[d]);
                 const XgmBlockHdr hh = hdr[src];
-                const uint32_t nterms = mq->nterms, sp = mq->src_pos;
+                const uint32_t nterms = mq->nterms, sp = mq->src_pos, unw = mq->unweighted;
                 /* MultiAndPostList::get_weight: result += plist[i]->get_weight(), in plist order
                  * (multiandpostlist.cc:149-159); a weighted range source is the child at position src_pos */
                 if (sp == 0) acc = mq->src_weight;
-                acc = __dadd_rn(acc, bm25_sumpart(mq->terms[0].termweight, mq, unpack_gl(p.tfs, hh.tf_off, pos, XGM_HDR_TF_BITS(hh.meta)), dlen));
+                if (!(unw & 1u))
+                    acc = __dadd_rn(acc, bm25_sumpart(mq->terms[0].termweight, mq, unpack_gl(p.tfs, hh.tf_off, pos, XGM_HDR_TF_BITS(hh.meta)), dlen));
                 for (uint32_t j = 1; j < nterms; ++j) {
                     if (sp == j) acc = __dadd_rn(acc, mq->src_weight);
+                    if (unw >> j & 1u) continue;
                     const uint32_t r = bitmap_rank(p, mq->terms[j], d);
                     const XgmBlockHdr bh = hdr[mq->terms[j].blk_begin + (r >> 7)];
                     const uint32_t tfj = unpack_gl(p.tfs, bh.tf_off, r & 127u, XGM_HDR_TF_BITS(bh.meta));
