@@ -340,7 +340,11 @@ xgm_status xgm_merge_msets(const uint32_t* const* docids, const double* const* w
  * nparts*nq*stride records laid out [part][query][rank], gathered_counts the per-part result records
  * (the buffer xgm_search_device_results returns as `counts`, 32 bytes per query, first u32 = n);
  * local docids are unsharded on the fly (part p = shard p of nparts). Outputs: [nq][k] weights and
- * docids, [nq] counts. Relevance order only. */
+ * docids, [nq] counts. Relevance order only.  A query that any part lost (its shard's overflow pool could
+ * not take a tie mass: xgm_search_wait reports XGM_E_UNIMPLEMENTED for it) gets count UINT32_MAX and no
+ * records, never a merge without that shard's documents; the other queries are unaffected.  A query declined
+ * because of its shape is declined on every shard alike and merges with count 0.
+ * Limits: k <= stride, nparts <= 64, nparts * k * 12 <= 200 KiB (the kernel's shared memory). */
 xgm_status xgm_merge_topk_device(const void* gathered_weights, const void* gathered_docids,
                                  const void* gathered_counts, uint32_t nparts, uint32_t nq, uint32_t stride,
                                  uint32_t k, void* out_weights, void* out_docids, void* out_counts,

@@ -2313,7 +2313,9 @@ __global__ void __launch_bounds__(TOPK_THREADS) xgm_topk_kernel(XgmKernelParams 
  * records: one CTA per query merges the nparts sorted lists under (weight desc, docid asc) with docids
  * mapped through unshard() (backends/multi.h:66-70).  Every part arrives sorted in that very order
  * (unshard is monotone within a part), so the rank of a record is its index in its own part plus, for
- * every other part, the number of records there that rank before it — a binary search each. */
+ * every other part, the number of records there that rank before it — a binary search each.  A part whose
+ * record is LOST or PENDING holds no answer for the query, so the query gets count UINT32_MAX and no records
+ * rather than a merge that silently misses that shard's documents. */
 #define XGM_MERGE_MAX_PARTS 64
 __global__ void __launch_bounds__(256) xgm_merge_kernel(const double* __restrict__ gw, const uint32_t* __restrict__ gd,
                                                         const XgmDevResult* __restrict__ ginfo, size_t part_w,
@@ -2326,11 +2328,16 @@ __global__ void __launch_bounds__(256) xgm_merge_kernel(const double* __restrict
     __shared__ uint32_t s_cnt[XGM_MERGE_MAX_PARTS];
     const uint32_t qi = blockIdx.x;
     /* part strides are in bytes: the parts are either three gathered arrays or whole result slabs */
+    uint32_t lost = 0;
     for (uint32_t part = threadIdx.x; part < nparts; part += blockDim.x) {
         const XgmDevResult* pi = reinterpret_cast<const XgmDevResult*>(reinterpret_cast<const unsigned char*>(ginfo) + part * part_info);
         s_cnt[part] = min(pi[qi].n, k);
+        lost |= pi[qi].flags & (XGM_RES_LOST | XGM_RES_PENDING);
     }
-    __syncthreads();
+    if (__syncthreads_or(lost)) {
+        if (threadIdx.x == 0) out_n[qi] = UINT32_MAX;
+        return;
+    }
     const size_t off = (size_t)qi * stride;
     for (uint32_t x = threadIdx.x; x < nparts * k; x += blockDim.x) {
         const uint32_t part = x / k, i = x - part * k;
