@@ -306,6 +306,10 @@ xgm_status xgm_search_device_results(xgm_searcher*, void** weights, void** docid
  * handler.cc:1540-1556's per-shard prepared MSets). */
 xgm_status xgm_search_device_slab(xgm_searcher*, void** base, uint64_t* bytes, uint64_t* off_docids,
                                   uint64_t* off_counts, uint32_t* stride);
+/* The slab's fourth region, after the per-query records: the records' sort keys u64[nq*max_topk] at *off_keys
+ * (256-byte aligned like the other regions), what xgm_search_wait returns as sort_keys for a value-sorted query.
+ * A relevance-ordered query's keys there are unspecified. */
+xgm_status xgm_search_device_slab_keys(xgm_searcher*, uint64_t* off_keys);
 /* Multi-GPU use: leave the batch's results in the device slab only — xgm_search_submit* then skips the
  * device→host copies and xgm_search_wait only synchronises (its output arguments may be NULL).  The caller
  * exchanges and merges the slabs on the device and copies the merged MSets itself. */
@@ -340,7 +344,7 @@ xgm_status xgm_merge_msets(const uint32_t* const* docids, const double* const* w
  * nparts*nq*stride records laid out [part][query][rank], gathered_counts the per-part result records
  * (the buffer xgm_search_device_results returns as `counts`, 32 bytes per query, first u32 = n);
  * local docids are unsharded on the fly (part p = shard p of nparts). Outputs: [nq][k] weights and
- * docids, [nq] counts. Relevance order only.  A query that any part lost (its shard's overflow pool could
+ * docids, [nq] counts. Relevance order (xgm_merge_mset_device_slab takes every order).  A query that any part lost (its shard's overflow pool could
  * not take a tie mass: xgm_search_wait reports XGM_E_UNIMPLEMENTED for it) gets count UINT32_MAX and no
  * records, never a merge without that shard's documents; the other queries are unaffected.  A query declined
  * because of its shape is declined on every shard alike and merges with count 0.
@@ -355,6 +359,28 @@ xgm_status xgm_merge_topk_device_slab(const void* gathered, uint64_t slab_bytes,
                                       uint64_t off_counts, uint32_t nparts, uint32_t nq, uint32_t stride,
                                       uint32_t k, void* out_weights, void* out_docids, void* out_counts,
                                       void* cuda_stream);
+/* The merge of gathered result slabs under each query's own order, with first > 0: Matcher::merge_mset under
+ * Multi_MultiValueKeyMaker's comparator, as xgm_merge_msets does on the host.  off_keys is the slab's keys region
+ * (xgm_search_device_slab_keys).  orders: device u8[nq], bits 0-1 the query's XGM_SORT_*, bit 2 its sort_reverse;
+ * NULL orders every query by relevance and reads no keys.  The comparator, ties broken by ascending docid:
+ *   XGM_SORT_VAL      key, docid (the weight is not compared);   XGM_SORT_VAL_REL  key, weight, docid;
+ *   XGM_SORT_REL_VAL  weight, key, docid;                         XGM_SORT_REL      weight, docid.
+ * Keys compare as unsigned 64-bit integers, ascending, or descending under reverse, which flips only the key.
+ * Weights compare descending.  Each part gives its first min(n, first + maxitems) records (so every shard is
+ * searched for ranks [0, first + maxitems)); merged ranks [first, first + maxitems) are written to
+ * out_weights/out_docids/out_keys [nq][maxitems] and out_counts [nq] holds min(max(total - first, 0), maxitems).
+ * Keys are written for queries whose order compares them; the rows of other queries in out_keys are not written.
+ * A part that lost the query (as for xgm_merge_topk_device) or an order byte above 7 gives that query count
+ * UINT32_MAX and no records; nothing is written past a count.  Each part must arrive sorted in its query's order,
+ * as the searcher leaves it.
+ * Limits: maxitems >= 1, first + maxitems <= stride, nparts <= 64,
+ * nparts * (first + maxitems) * 20 <= 200 KiB (the kernel's shared memory); 8-byte aligned offsets, regions
+ * weights | docids | records | keys in that order, each holding nq*stride records. */
+xgm_status xgm_merge_mset_device_slab(const void* gathered, uint64_t slab_bytes, uint64_t off_docids,
+                                      uint64_t off_counts, uint64_t off_keys, const uint8_t* orders,
+                                      uint32_t nparts, uint32_t nq, uint32_t stride, uint32_t first,
+                                      uint32_t maxitems, void* out_weights, void* out_docids,
+                                      void* out_keys, void* out_counts, void* cuda_stream);
 
 #ifdef __cplusplus
 }

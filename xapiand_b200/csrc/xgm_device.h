@@ -119,9 +119,22 @@ cudaError_t xgm_launch_coarse(const uint32_t* bitmaps, size_t ncoarse, uint32_t*
 cudaError_t xgm_launch_decode(const XgmKernelParams& p, uint32_t blk_begin, uint32_t nblocks, uint32_t* out_d,
                               uint32_t* out_w, cudaStream_t s);
 size_t xgm_topk_smem_bytes(uint32_t keep_cap);
-cudaError_t xgm_launch_merge(const double* gw, const uint32_t* gd, const XgmDevResult* ginfo, size_t part_w, size_t part_d,
-                             size_t part_info, uint32_t nparts, uint32_t nq, uint32_t stride, uint32_t k, double* out_w, uint32_t* out_d, uint32_t* out_n,
-                             cudaStream_t s);
+/* xgm_merge_kernel's inputs: nparts gathered parts, part p of each array at base + p * part_* bytes, [query][rank]
+ * records of `stride` per query; outputs [nq][maxitems] records and [nq] counts. */
+struct XgmMergeArgs {
+    const double* gw;
+    const uint32_t* gd;
+    const uint64_t* gk;          /* sort keys; null: no order reads them (then out_k is not written) */
+    const XgmDevResult* ginfo;
+    size_t part_w, part_d, part_k, part_info;
+    const uint8_t* orders;       /* [nq]: bits 0-1 XGM_SORT_*, bit 2 reverse; null: relevance for every query */
+    uint32_t nparts, nq, stride, first, maxitems;
+    double* out_w;
+    uint32_t* out_d;
+    uint64_t* out_k;
+    uint32_t* out_n;
+};
+cudaError_t xgm_launch_merge(const XgmMergeArgs& a, cudaStream_t s);
 int xgm_and_occupancy_blocks_per_sm();
 
 #endif

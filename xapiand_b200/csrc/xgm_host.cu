@@ -1050,8 +1050,8 @@ struct xgm_searcher {
     uint32_t* d_out_d = nullptr;
     uint64_t* d_out_k = nullptr;
     XgmDevResult* d_info = nullptr;
-    unsigned char* d_slab = nullptr; /* d_out_w | d_out_d | d_info in one allocation: one all-gather moves a shard's MSets */
-    size_t slab_bytes = 0, slab_off_d = 0, slab_off_info = 0;
+    unsigned char* d_slab = nullptr; /* d_out_w | d_out_d | d_info | d_out_k in one allocation: one all-gather moves a shard's MSets */
+    size_t slab_bytes = 0, slab_off_d = 0, slab_off_info = 0, slab_off_k = 0;
     /* last batch */
     std::vector<PlannedQuery> plan;
     uint32_t nq = 0;
@@ -1111,7 +1111,7 @@ extern "C" void xgm_searcher_free(xgm_searcher* s) {
     cudaFreeHost(s->h_out_k); cudaFreeHost(s->h_info); cudaFreeHost(s->h_raise); cudaFree(s->d_raise); cudaFreeHost(s->h_qstate); cudaFreeHost(s->h_tileq); cudaFree(s->d_tileq);
     cudaFree(s->d_queries); s->and_list.release(); s->or_list.release(); s->bm_list.release();
     cudaFree(s->d_ctrl); cudaFree(s->d_topk_list); cudaFree(s->d_match_w); cudaFree(s->d_match_d);
-    cudaFree(s->d_match_k); cudaFree(s->d_pool_w); cudaFree(s->d_pool_d); cudaFree(s->d_pool_k); cudaFree(s->d_slab); cudaFree(s->d_out_k);
+    cudaFree(s->d_match_k); cudaFree(s->d_pool_w); cudaFree(s->d_pool_d); cudaFree(s->d_pool_k); cudaFree(s->d_slab);
     if (s->ev0) cudaEventDestroy(s->ev0);
     if (s->ev1) cudaEventDestroy(s->ev1);
     if (s->ev2) cudaEventDestroy(s->ev2);
@@ -1180,13 +1180,14 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
         auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
         s->slab_off_d = up(ns * 8);
         s->slab_off_info = s->slab_off_d + up(ns * 4);
-        s->slab_bytes = s->slab_off_info + up(nq * sizeof(XgmDevResult));
+        s->slab_off_k = s->slab_off_info + up(nq * sizeof(XgmDevResult));
+        s->slab_bytes = s->slab_off_k + up(ns * 8);
         CUDA_TRY(cudaMalloc(&s->d_slab, s->slab_bytes));
         s->d_out_w = reinterpret_cast<double*>(s->d_slab);
         s->d_out_d = reinterpret_cast<uint32_t*>(s->d_slab + s->slab_off_d);
         s->d_info = reinterpret_cast<XgmDevResult*>(s->d_slab + s->slab_off_info);
+        s->d_out_k = reinterpret_cast<uint64_t*>(s->d_slab + s->slab_off_k);
     }
-    CUDA_TRY(cudaMalloc(&s->d_out_k, ns * 8));
     /* overflow pool: room for the tie mass of a few pathological queries per batch (doccount entries at least) */
     s->pool_total = std::max<uint32_t>(1u << 20, std::min<uint32_t>(1u << 25, 2 * ix->doccount + (1u << 16)));
     if (const char* e = getenv("XGM_POOL_ENTRIES")) s->pool_total = (uint32_t)strtoul(e, nullptr, 10);
@@ -2244,6 +2245,12 @@ extern "C" xgm_status xgm_search_device_slab(xgm_searcher* s, void** base, uint6
     return XGM_OK;
 }
 
+extern "C" xgm_status xgm_search_device_slab_keys(xgm_searcher* s, uint64_t* off_keys) {
+    if (!s || !off_keys) return fail(XGM_E_INVALID, "null argument");
+    *off_keys = s->slab_off_k;
+    return XGM_OK;
+}
+
 extern "C" xgm_status xgm_search_last_stats(xgm_searcher* s, xgm_batch_stats* out) {
     if (!s || !out) return fail(XGM_E_INVALID, "null argument");
     if (!s->pending && s->nq) {
@@ -2333,17 +2340,38 @@ extern "C" xgm_status xgm_merge_msets(const uint32_t* const* docids, const doubl
     return XGM_OK;
 }
 
+/* The relevance-order entry points below: no orders, no keys, first = 0, maxitems = k. */
+static XgmMergeArgs rel_merge_args(uint32_t nparts, uint32_t nq, uint32_t stride, uint32_t k, void* out_w, void* out_d,
+                                   void* out_n) {
+    XgmMergeArgs a{};
+    a.nparts = nparts; a.nq = nq; a.stride = stride; a.first = 0; a.maxitems = k;
+    a.out_w = static_cast<double*>(out_w); a.out_d = static_cast<uint32_t*>(out_d); a.out_n = static_cast<uint32_t*>(out_n);
+    return a;
+}
+
 extern "C" xgm_status xgm_merge_topk_device(const void* gw, const void* gd, const void* ginfo, uint32_t nparts, uint32_t nq,
                                             uint32_t stride, uint32_t k, void* out_w, void* out_d, void* out_n,
                                             void* cuda_stream) {
     if (!gw || !gd || !ginfo || !out_w || !out_d || !out_n || nparts == 0 || nq == 0 || k == 0 || k > stride)
         return fail(XGM_E_INVALID, "bad arguments");
     if ((size_t)nparts * k * 12 > 200 * 1024 || nparts > 64) return fail(XGM_E_INVALID, "nparts*k too large for the merge kernel");
-    CUDA_TRY(xgm_launch_merge(static_cast<const double*>(gw), static_cast<const uint32_t*>(gd),
-                              static_cast<const XgmDevResult*>(ginfo), (size_t)nq * stride * 8, (size_t)nq * stride * 4,
-                              (size_t)nq * sizeof(XgmDevResult), nparts, nq, stride, k, static_cast<double*>(out_w),
-                              static_cast<uint32_t*>(out_d), static_cast<uint32_t*>(out_n),
-                              static_cast<cudaStream_t>(cuda_stream)));
+    XgmMergeArgs a = rel_merge_args(nparts, nq, stride, k, out_w, out_d, out_n);
+    a.gw = static_cast<const double*>(gw); a.gd = static_cast<const uint32_t*>(gd);
+    a.ginfo = static_cast<const XgmDevResult*>(ginfo);
+    a.part_w = (size_t)nq * stride * 8; a.part_d = (size_t)nq * stride * 4; a.part_info = (size_t)nq * sizeof(XgmDevResult);
+    CUDA_TRY(xgm_launch_merge(a, static_cast<cudaStream_t>(cuda_stream)));
+    return XGM_OK;
+}
+
+/* Checks of a gathered slab layout shared by both slab entry points: 8-byte aligned offsets, regions in slab order
+ * (weights | docids | records | keys when off_keys != 0) each large enough for nq*stride records. */
+static xgm_status check_slab_layout(uint64_t slab_bytes, uint64_t off_docids, uint64_t off_counts, uint64_t off_keys,
+                                    bool keys, uint32_t nq, uint32_t stride) {
+    if ((slab_bytes | off_docids | off_counts | off_keys) & 7) return fail(XGM_E_INVALID, "slab offsets must be 8-byte aligned");
+    const uint64_t ns = (uint64_t)nq * stride, end_counts = off_counts + (uint64_t)nq * sizeof(XgmDevResult);
+    if (off_docids < ns * 8 || off_counts < off_docids + ns * 4 || slab_bytes < end_counts ||
+        (keys && (off_keys < end_counts || slab_bytes < off_keys + ns * 8)))
+        return fail(XGM_E_INVALID, "slab layout too small for nq*stride records");
     return XGM_OK;
 }
 
@@ -2352,15 +2380,40 @@ extern "C" xgm_status xgm_merge_topk_device_slab(const void* gathered, uint64_t 
                                                  uint32_t k, void* out_w, void* out_d, void* out_n, void* cuda_stream) {
     if (!gathered || !out_w || !out_d || !out_n || nparts == 0 || nq == 0 || k == 0 || k > stride)
         return fail(XGM_E_INVALID, "bad arguments");
-    if ((slab_bytes | off_docids | off_counts) & 7) return fail(XGM_E_INVALID, "slab offsets must be 8-byte aligned");
-    if (off_docids < (uint64_t)nq * stride * 8 || off_counts < off_docids + (uint64_t)nq * stride * 4 ||
-        slab_bytes < off_counts + (uint64_t)nq * sizeof(XgmDevResult))
-        return fail(XGM_E_INVALID, "slab layout too small for nq*stride records");
+    xgm_status st = check_slab_layout(slab_bytes, off_docids, off_counts, 0, false, nq, stride);
+    if (st != XGM_OK) return st;
     if ((size_t)nparts * k * 12 > 200 * 1024 || nparts > 64) return fail(XGM_E_INVALID, "nparts*k too large for the merge kernel");
     const unsigned char* g = static_cast<const unsigned char*>(gathered);
-    CUDA_TRY(xgm_launch_merge(reinterpret_cast<const double*>(g), reinterpret_cast<const uint32_t*>(g + off_docids),
-                              reinterpret_cast<const XgmDevResult*>(g + off_counts), slab_bytes, slab_bytes, slab_bytes,
-                              nparts, nq, stride, k, static_cast<double*>(out_w), static_cast<uint32_t*>(out_d),
-                              static_cast<uint32_t*>(out_n), static_cast<cudaStream_t>(cuda_stream)));
+    XgmMergeArgs a = rel_merge_args(nparts, nq, stride, k, out_w, out_d, out_n);
+    a.gw = reinterpret_cast<const double*>(g); a.gd = reinterpret_cast<const uint32_t*>(g + off_docids);
+    a.ginfo = reinterpret_cast<const XgmDevResult*>(g + off_counts);
+    a.part_w = a.part_d = a.part_info = slab_bytes;
+    CUDA_TRY(xgm_launch_merge(a, static_cast<cudaStream_t>(cuda_stream)));
+    return XGM_OK;
+}
+
+extern "C" xgm_status xgm_merge_mset_device_slab(const void* gathered, uint64_t slab_bytes, uint64_t off_docids,
+                                                 uint64_t off_counts, uint64_t off_keys, const uint8_t* orders,
+                                                 uint32_t nparts, uint32_t nq, uint32_t stride, uint32_t first,
+                                                 uint32_t maxitems, void* out_weights, void* out_docids,
+                                                 void* out_keys, void* out_counts, void* cuda_stream) {
+    if (!gathered || !out_weights || !out_docids || !out_keys || !out_counts || nparts == 0 || nq == 0 || maxitems == 0 ||
+        (uint64_t)first + maxitems > stride)
+        return fail(XGM_E_INVALID, "bad arguments");
+    xgm_status st = check_slab_layout(slab_bytes, off_docids, off_counts, off_keys, true, nq, stride);
+    if (st != XGM_OK) return st;
+    if ((uint64_t)nparts * (first + maxitems) * 20 > 200 * 1024 || nparts > 64)
+        return fail(XGM_E_INVALID, "nparts*(first+maxitems) too large for the merge kernel");
+    const unsigned char* g = static_cast<const unsigned char*>(gathered);
+    XgmMergeArgs a{};
+    a.gw = reinterpret_cast<const double*>(g); a.gd = reinterpret_cast<const uint32_t*>(g + off_docids);
+    a.gk = orders ? reinterpret_cast<const uint64_t*>(g + off_keys) : nullptr; /* no orders: relevance, no keys */
+    a.ginfo = reinterpret_cast<const XgmDevResult*>(g + off_counts);
+    a.part_w = a.part_d = a.part_k = a.part_info = slab_bytes;
+    a.orders = orders;
+    a.nparts = nparts; a.nq = nq; a.stride = stride; a.first = first; a.maxitems = maxitems;
+    a.out_w = static_cast<double*>(out_weights); a.out_d = static_cast<uint32_t*>(out_docids);
+    a.out_k = static_cast<uint64_t*>(out_keys); a.out_n = static_cast<uint32_t*>(out_counts);
+    CUDA_TRY(xgm_launch_merge(a, static_cast<cudaStream_t>(cuda_stream)));
     return XGM_OK;
 }

@@ -2310,83 +2310,92 @@ __global__ void __launch_bounds__(TOPK_THREADS) xgm_topk_kernel(XgmKernelParams 
 /* ------------------------------------------------------------------ multi-shard merge */
 
 /* Matcher::merge_mset (matcher.cc:653-782) on the device, after an all-gather of the per-GPU top-k
- * records: one CTA per query merges the nparts sorted lists under (weight desc, docid asc) with docids
- * mapped through unshard() (backends/multi.h:66-70).  Every part arrives sorted in that very order
+ * records: one CTA per query merges the nparts sorted lists under the query's order (ranks_before, the
+ * reference's msetcmp: relevance, value, value then relevance, relevance then value, reverse on the value) with
+ * docids mapped through unshard() (backends/multi.h:66-70).  Every part arrives sorted in that very order
  * (unshard is monotone within a part), so the rank of a record is its index in its own part plus, for
- * every other part, the number of records there that rank before it — a binary search each.  A part whose
- * record is LOST or PENDING holds no answer for the query, so the query gets count UINT32_MAX and no records
- * rather than a merge that silently misses that shard's documents. */
+ * every other part, the number of records there that rank before it — a binary search each.  Each part gives
+ * its first first + maxitems records; merged ranks [first, first + maxitems) are written.  A part whose record
+ * is LOST or PENDING holds no answer for the query, and an order byte above 7 names no order, so such a query
+ * gets count UINT32_MAX and no records rather than a merge that silently misses that shard's documents.  The
+ * order is the same for the whole CTA, so its branches do not diverge. */
 #define XGM_MERGE_MAX_PARTS 64
-__global__ void __launch_bounds__(256) xgm_merge_kernel(const double* __restrict__ gw, const uint32_t* __restrict__ gd,
-                                                        const XgmDevResult* __restrict__ ginfo, size_t part_w,
-                                                        size_t part_d, size_t part_info, uint32_t nparts,
-                                                        uint32_t nq, uint32_t stride, uint32_t k, double* out_w,
-                                                        uint32_t* out_d, uint32_t* out_n) {
+/* 8 CTAs per SM: 32 registers, the full 2048 threads wherever shared memory allows it (no spills) */
+__global__ void __launch_bounds__(256, 8) xgm_merge_kernel(const XgmMergeArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    double* sw = reinterpret_cast<double*>(smem_raw);
-    uint32_t* sd = reinterpret_cast<uint32_t*>(sw + (size_t)nparts * k);
     __shared__ uint32_t s_cnt[XGM_MERGE_MAX_PARTS];
     const uint32_t qi = blockIdx.x;
-    /* part strides are in bytes: the parts are either three gathered arrays or whole result slabs */
-    uint32_t lost = 0;
-    for (uint32_t part = threadIdx.x; part < nparts; part += blockDim.x) {
-        const XgmDevResult* pi = reinterpret_cast<const XgmDevResult*>(reinterpret_cast<const unsigned char*>(ginfo) + part * part_info);
-        s_cnt[part] = min(pi[qi].n, k);
+    const uint32_t order = a.orders ? a.orders[qi] : 0u;
+    const uint32_t sort_by = order & 3u, reverse = (order >> 2) & 1u;
+    const bool keyed = a.gk != nullptr && sort_by != 0u; /* XGM_SORT_REL compares no key */
+    const uint32_t m = a.first + a.maxitems; /* records taken from each part, and the last merged rank + 1 */
+    const size_t nrec = (size_t)a.nparts * m;
+    double* sw = reinterpret_cast<double*>(smem_raw);
+    uint64_t* sk = reinterpret_cast<uint64_t*>(sw + nrec);
+    uint32_t* sd = reinterpret_cast<uint32_t*>(sk + (a.gk ? nrec : 0));
+    /* part strides are in bytes: the parts are either gathered arrays or whole result slabs */
+    uint32_t lost = order > 7u;
+    for (uint32_t part = threadIdx.x; part < a.nparts; part += blockDim.x) {
+        const XgmDevResult* pi = reinterpret_cast<const XgmDevResult*>(reinterpret_cast<const unsigned char*>(a.ginfo) + part * a.part_info);
+        s_cnt[part] = min(pi[qi].n, m);
         lost |= pi[qi].flags & (XGM_RES_LOST | XGM_RES_PENDING);
     }
     if (__syncthreads_or(lost)) {
-        if (threadIdx.x == 0) out_n[qi] = UINT32_MAX;
+        if (threadIdx.x == 0) a.out_n[qi] = UINT32_MAX;
         return;
     }
-    const size_t off = (size_t)qi * stride;
-    for (uint32_t x = threadIdx.x; x < nparts * k; x += blockDim.x) {
-        const uint32_t part = x / k, i = x - part * k;
+    const size_t off = (size_t)qi * a.stride;
+    for (uint32_t x = threadIdx.x; x < nrec; x += blockDim.x) {
+        const uint32_t part = x / m, i = x - part * m;
         if (i < s_cnt[part]) {
-            const double* pw = reinterpret_cast<const double*>(reinterpret_cast<const unsigned char*>(gw) + part * part_w);
-            const uint32_t* pd = reinterpret_cast<const uint32_t*>(reinterpret_cast<const unsigned char*>(gd) + part * part_d);
+            const double* pw = reinterpret_cast<const double*>(reinterpret_cast<const unsigned char*>(a.gw) + part * a.part_w);
+            const uint32_t* pd = reinterpret_cast<const uint32_t*>(reinterpret_cast<const unsigned char*>(a.gd) + part * a.part_d);
             sw[x] = pw[off + i];
-            sd[x] = (pd[off + i] - 1u) * nparts + part + 1u;
+            sd[x] = (pd[off + i] - 1u) * a.nparts + part + 1u;
+            if (keyed) sk[x] = reinterpret_cast<const uint64_t*>(reinterpret_cast<const unsigned char*>(a.gk) + part * a.part_k)[off + i];
         }
     }
     __syncthreads();
     uint32_t total = 0;
-    for (uint32_t part = 0; part < nparts; ++part) total += s_cnt[part];
-    for (uint32_t x = threadIdx.x; x < nparts * k; x += blockDim.x) {
-        const uint32_t part = x / k, i = x - part * k;
+    for (uint32_t part = 0; part < a.nparts; ++part) total += s_cnt[part];
+    const size_t ooff = (size_t)qi * a.maxitems;
+    for (uint32_t x = threadIdx.x; x < nrec; x += blockDim.x) {
+        const uint32_t part = x / m, i = x - part * m;
         if (i >= s_cnt[part]) continue;
         const double wi = sw[x];
         const uint32_t di = sd[x];
+        const uint64_t ki = keyed ? sk[x] : 0ull;
         uint32_t rank = i;
-        for (uint32_t o = 0; o < nparts && rank < k; ++o) {
+        for (uint32_t o = 0; o < a.nparts && rank < m; ++o) {
             if (o == part) continue;
-            const double* ow = sw + (size_t)o * k;
-            const uint32_t* od = sd + (size_t)o * k;
-            uint32_t lo = 0, hi = s_cnt[o]; /* first record of part o that does not rank before (wi, di) */
+            const size_t ob = (size_t)o * m;
+            uint32_t lo = 0, hi = s_cnt[o]; /* first record of part o that does not rank before record x */
             while (lo < hi) {
                 const uint32_t mid = (lo + hi) >> 1;
-                const double wm = ow[mid];
-                if (wm > wi || (wm == wi && od[mid] < di)) lo = mid + 1; else hi = mid;
+                if (ranks_before(sort_by, reverse, sw[ob + mid], sd[ob + mid], keyed ? sk[ob + mid] : 0ull, wi, di, ki))
+                    lo = mid + 1;
+                else
+                    hi = mid;
             }
             rank += lo;
         }
-        if (rank < k) {
-            out_w[(size_t)qi * k + rank] = wi;
-            out_d[(size_t)qi * k + rank] = di;
+        if (rank >= a.first && rank < m) {
+            a.out_w[ooff + rank - a.first] = wi;
+            a.out_d[ooff + rank - a.first] = di;
+            if (keyed) a.out_k[ooff + rank - a.first] = ki;
         }
     }
-    if (threadIdx.x == 0) out_n[qi] = total < k ? total : k;
+    if (threadIdx.x == 0) a.out_n[qi] = total > a.first ? min(total - a.first, a.maxitems) : 0u;
 }
 
-cudaError_t xgm_launch_merge(const double* gw, const uint32_t* gd, const XgmDevResult* ginfo, size_t part_w, size_t part_d,
-                             size_t part_info, uint32_t nparts, uint32_t nq, uint32_t stride, uint32_t k, double* out_w, uint32_t* out_d, uint32_t* out_n,
-                             cudaStream_t s) {
-    if (nparts > XGM_MERGE_MAX_PARTS) return cudaErrorInvalidValue;
-    size_t smem = (size_t)nparts * k * 12;
+cudaError_t xgm_launch_merge(const XgmMergeArgs& a, cudaStream_t s) {
+    if (a.nparts > XGM_MERGE_MAX_PARTS) return cudaErrorInvalidValue;
+    const size_t smem = (size_t)a.nparts * (a.first + a.maxitems) * (a.gk ? 20 : 12);
     if (smem > 48 * 1024) {
         cudaError_t e = optin_smem((const void*)xgm_merge_kernel, 0, smem);
         if (e != cudaSuccess) return e;
     }
-    xgm_merge_kernel<<<nq, 256, smem, s>>>(gw, gd, ginfo, part_w, part_d, part_info, nparts, nq, stride, k, out_w, out_d, out_n);
+    xgm_merge_kernel<<<a.nq, 256, smem, s>>>(a);
     return cudaGetLastError();
 }
 

@@ -8,7 +8,10 @@
 
 Works with any backend (NCCL on GPUs, gloo in the CPU tests); the device-resident variant used for the
 throughput numbers lives in bench.py (statistics through xapiand_b200/shm_exchange.py on one node, one all-to-all of
-per-query-slice top-k + xgm_merge_topk_device).
+per-query-slice top-k + xgm_merge_topk_device, which merges by relevance).  A device path for value-sorted batches
+exchanges whole result slabs, sort keys included, and merges them with xgm.merge_device_slabs
+(xgm_merge_mset_device_slab: every sort order, reverse and first, records only); merge_over_ranks below is the
+full merge, statistics included.
 """
 from __future__ import annotations
 

@@ -30,9 +30,9 @@ EXPORTS = [
     "xgm_index_load_flat", "xgm_index_close", "xgm_index_info_get", "xgm_term_stats_get",
     "xgm_index_decode_term", "xgm_index_copy_doclengths", "xgm_searcher_new", "xgm_searcher_free", "xgm_search_submit", "xgm_search_wait",
     "xgm_search_submit_async", "xgm_search_launched", "xgm_search_batch", "xgm_search", "xgm_search_replay",
-    "xgm_search_device_results", "xgm_search_device_slab",
+    "xgm_search_device_results", "xgm_search_device_slab", "xgm_search_device_slab_keys",
     "xgm_searcher_stream", "xgm_search_last_stats", "xgm_unshard", "xgm_merge_msets", "xgm_merge_topk_device",
-    "xgm_merge_topk_device_slab",
+    "xgm_merge_topk_device_slab", "xgm_merge_mset_device_slab",
     "xgm_builder_add_value_slot_serialised", "xgm_builder_set_revision", "xgm_index_value_freq",
     "xgm_value_key", "xgm_value_key_bytes", "xgm_sort_key_bytes", "xgm_term_stats_many",
     "xgm_index_open", "xgm_glass_revision", "xgm_glass_export_flat", "xgm_searcher_set_results_on_device",
@@ -159,8 +159,12 @@ def lib():
                                             C.POINTER(C.c_void_p), C.POINTER(C.c_uint32)]
     L.xgm_search_device_slab.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
                                          C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
+    L.xgm_search_device_slab_keys.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.xgm_merge_topk_device_slab.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32,
                                              C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.xgm_merge_mset_device_slab.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p,
+                                             C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.xgm_searcher_stream.argtypes = [C.c_void_p]
     L.xgm_searcher_stream.restype = C.c_void_p
     L.xgm_search_last_stats.argtypes = [C.c_void_p, C.POINTER(BatchStats)]
@@ -571,6 +575,12 @@ class Searcher:
         _check(lib().xgm_search_device_slab(self._h, C.byref(b), C.byref(n), C.byref(od), C.byref(oc), C.byref(s)))
         return b.value, n.value, od.value, oc.value, s.value
 
+    def device_slab_keys(self) -> int:
+        """Offset of the result slab's sort-key region (u64 per record, stride as device_slab's)."""
+        ok = C.c_uint64()
+        _check(lib().xgm_search_device_slab_keys(self._h, C.byref(ok)))
+        return ok.value
+
 
 def unshard(docids: np.ndarray, shard: int, nshards: int) -> np.ndarray:
     d = np.ascontiguousarray(docids, np.uint32).copy()
@@ -611,6 +621,33 @@ def merge_msets(parts: Sequence[MSet], first: int, maxitems: int, sort_by: int =
     return MSet(od[:oi.n], ow[:oi.n], ok[:oi.n], first, oi.matches_lower_bound, oi.matches_estimated,
                 oi.matches_upper_bound, oi.max_possible, oi.max_attained, oi.percent_scale_factor,
                 oi.exact_matches, oi.status, oi.flags)
+
+
+def merge_device_slabs(gathered, slab_bytes: int, off_docids: int, off_counts: int, off_keys: int, orders,
+                       nparts: int, nq: int, stride: int, first: int, maxitems: int, stream=None):
+    """xgm_merge_mset_device_slab over nparts gathered result slabs (a CUDA tensor, slab p at byte p * slab_bytes):
+    Matcher::merge_mset of every query under its own order.  orders: a CUDA uint8 tensor [nq] (bits 0-1 the query's
+    SORT_*, bit 2 its sort_reverse) or None for relevance order everywhere.  Returns (counts, docids, weights, keys)
+    as CUDA tensors: int32 [nq] (UINT32_MAX, i.e. -1, for a query some part lost), int32 [nq, maxitems] (the
+    uint32 docids' bits), float64 and int64 [nq, maxitems] (the uint64 keys' bits); entries past a query's count,
+    and the keys of queries ordered by relevance, are zero.  Runs on `stream` (a cudaStream_t as int) or the
+    current torch stream."""
+    import torch
+    dev = gathered.device
+    counts = torch.zeros(nq, dtype=torch.int32, device=dev)
+    docids = torch.zeros((nq, maxitems), dtype=torch.int32, device=dev)
+    weights = torch.zeros((nq, maxitems), dtype=torch.float64, device=dev)
+    keys = torch.zeros((nq, maxitems), dtype=torch.int64, device=dev)
+    if orders is not None and (orders.dtype != torch.uint8 or orders.numel() != nq or not orders.is_contiguous()
+                               or orders.device != dev):
+        raise ValueError("orders must be a contiguous uint8 tensor of nq entries on the slabs' device")
+    if stream is None:
+        stream = torch.cuda.current_stream(dev).cuda_stream
+    _check(lib().xgm_merge_mset_device_slab(gathered.data_ptr(), slab_bytes, off_docids, off_counts, off_keys,
+                                            None if orders is None else orders.data_ptr(), nparts, nq, stride, first,
+                                            maxitems, weights.data_ptr(), docids.data_ptr(), keys.data_ptr(),
+                                            counts.data_ptr(), stream or None))
+    return counts, docids, weights, keys
 
 
 def value_key(b: bytes):
