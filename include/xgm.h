@@ -246,7 +246,9 @@ typedef struct xgm_mset_info {
  * buffer and check_at_least is at most first+maxitems+1 (Xapiand's default) or is never reached; for larger
  * match sets that were pruned on the device, or a check_at_least in between (where the reference's
  * min_weight lags, protomset.h:377-398), the lower bound / estimate are conservative (still valid
- * bounds) and this flag is set.  Docids, weights, max_possible,
+ * bounds) and this flag is set.  It is also set whenever the bounds of a query with an XGM_FILTER_VALUE_RANGE
+ * filter come from the query's structure: there the reference's estimate folds in ValueRangePostList's
+ * string-fraction estimate, which is not restated, while the lower and upper bounds are.  Docids, weights, max_possible,
  * max_attained, percent_scale_factor, the upper bound and exact_matches are always exact.
  * percent_scale_factor needs the number of subqueries matching the FIRST document in docid order that attains
  * max_attained (ProtoMSet::update_max_weight, protomset.h:174-183).  Where that document need not be among the

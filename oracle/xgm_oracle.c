@@ -571,6 +571,28 @@ static node_t and_pair_node(node_t a, node_t b, uint32_t doccount) {
     return r;
 }
 
+/* The range of OP_FILTER(base, range) as a MultiAndPostList child.  A MultipleValueRange source has termfreqs
+ * (min, est, max) = (0, vf, vf) (range.cc:457-464, api/postingsource.cc:201-214).  A stock OP_VALUE_RANGE has
+ * max = vf and min = vf when [lo, hi] covers every value in the slot, 0 otherwise (valuerangepostlist.cc:40-54,
+ * 145-148); its string-fraction estimate (valuerangepostlist.cc:70-130) is not restated and vf stands in for it. */
+static node_t range_child_node(const orc_index* ix, const orc_query* q) {
+    uint32_t vf = 0;
+    uint64_t lo = ~0ull, hi = 0;
+    if (ix->nvals0)
+        for (uint32_t d = 1; d <= ix->lastdocid; ++d) {
+            if (!ix->nvals0[d]) continue;
+            const uint64_t v = ix->vals0[3 * (size_t)d];
+            ++vf;
+            if (v < lo) lo = v;
+            if (v > hi) hi = v;
+        }
+    node_t r;
+    r.mn = q->filter == ORC_FILTER_VALUE_RANGE_MIN && vf && q->range_lo <= lo && hi <= q->range_hi ? vf : 0;
+    r.mx = r.est = vf;
+    r.maxw = 0.0;
+    return r;
+}
+
 static int list_contains(const uint32_t* d, uint32_t n, uint32_t did, uint32_t* where) {
     uint32_t lo = 0, hi = n;
     while (lo < hi) { uint32_t m = (lo + hi) / 2; if (d[m] < did) lo = m + 1; else hi = m; }
@@ -629,10 +651,10 @@ int orc_match(const orc_index* ix, const orc_query* qin, orc_mset* out) {
     double src_w = 0.0;
     if (q->op == ORC_OP_AND) {
         orc_and_order(len, n, order);
-        if (q->filter == ORC_FILTER_MULTI_RANGE && !(q->nfilter || q->nnot || q->nmaybe)) {
-            /* the range source is one more child, sorted in by its termfreq estimate = value_freq */
-            uint32_t vf = 0;
-            if (ix->nvals0) for (uint32_t d = 1; d <= ix->lastdocid; ++d) vf += ix->nvals0[d] != 0;
+        if (q->filter != ORC_FILTER_NONE && !(q->nfilter || q->nnot || q->nmaybe)) {
+            /* the range is one more child, sorted in by its termfreq estimate = value_freq */
+            const node_t src = range_child_node(ix, q);
+            const uint32_t vf = src.mx;
             uint32_t* cl = (uint32_t*)xcalloc(n + 1, 4);
             uint32_t* co = (uint32_t*)xcalloc(n + 1, 4);
             memcpy(cl, len, n * 4);
@@ -643,7 +665,7 @@ int orc_match(const orc_index* ix, const orc_query* qin, orc_mset* out) {
             for (uint32_t i = 0; i <= n; ++i) { if (co[i] == n) src_pos = k; else order[k++] = co[i]; }
             for (uint32_t i = 0; i <= n; ++i)
                 max_possible += co[i] == n ? (q->filter_weighted ? src_w * 1.7976931348623157e308 : 0.0) : maxpart[co[i]];
-            #define CH_MIN(i) (co[i] == n ? 0u : cl[co[i]])
+            #define CH_MIN(i) (co[i] == n ? src.mn : cl[co[i]])
             uint32_t sum = CH_MIN(0);
             if (sum) {
                 for (uint32_t i = 1; i <= n; ++i) {
@@ -709,6 +731,13 @@ int orc_match(const orc_index* ix, const orc_query* qin, orc_mset* out) {
         }
         max_possible = sm[0]; tf_min = smin[0]; tf_max = smax[0]; tf_est = (uint32_t)se[0];
         free(sm); free(se); free(smin); free(smax);
+        if (q->filter != ORC_FILTER_NONE) {
+            /* QueryFilter::postlist: MultiAndPostList of [OrPostList tree, range] (api/queryinternal.cc:2271-2283);
+             * the range weighs nothing, so max_possible stays the tree's */
+            node_t cur; cur.mn = tf_min; cur.mx = tf_max; cur.est = tf_est; cur.maxw = max_possible;
+            cur = and_pair_node(cur, range_child_node(ix, q), ix->doccount);
+            tf_min = cur.mn; tf_max = cur.mx; tf_est = cur.est;
+        }
     }
 
     /* §8(f)-1 groups around an AND base */
@@ -795,6 +824,15 @@ int orc_match(const orc_index* ix, const orc_query* qin, orc_mset* out) {
     for (uint32_t j = 0; j < n; ++j) nweighted += (!q->factors || q->factors[j] != 0.0) ? 1u : 0u;
     uint32_t total_subqs = nweighted + nm; /* api/queryinternal.cc:1053-1054 */
     if (q->filter_weighted && q->filter == ORC_FILTER_MULTI_RANGE) ++total_subqs; /* QueryPostingSource::postlist, factor != 0 */
+
+    /* a stock range covering every value of a slot that every document has is the all-documents list
+     * (QueryValueRange::postlist api/queryinternal.cc:1116-1124), whose LeafPostList has no Weight: it matches no
+     * subquery (leafpostlist.cc:88-91) */
+    int filter_subq = q->filter != ORC_FILTER_NONE;
+    if (q->filter == ORC_FILTER_VALUE_RANGE_MIN) {
+        const node_t r = range_child_node(ix, q);
+        if (r.mn != 0 && r.mn == ix->doccount) filter_subq = 0;
+    }
 
     uint64_t* pos = (uint64_t*)xcalloc(n, 8);
     double* stk = (double*)xcalloc(2 * (n + nm) + 2, 8);
@@ -910,7 +948,7 @@ int orc_match(const orc_index* ix, const orc_query* qin, orc_mset* out) {
              * (ValueRangePostList / ExternalPostList::count_matching_subqs return 1) although, being unweighted,
              * it is not one of the total_subqs (api/queryinternal.cc:1097-1098): percentages of filtered
              * queries are scaled by (n+1)/n */
-            if (q->filter != ORC_FILTER_NONE) ++subqs;
+            if (filter_subq) ++subqs;
             /* main loop, matcher/matcher.cc:482-536 */
             if (weight < P.min_weight) continue;
             res_t item;

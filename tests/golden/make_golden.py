@@ -63,27 +63,30 @@ def run_set(tag, ndocs, vocab, queries, nshards=1, twophase=False, values=False,
         shutil.rmtree(tmp, ignore_errors=True)
 
 
-def run_mv_set(tag, ndocs, vocab, queries, sparse=(7, 5), seed=12345):
+def run_mv_set(tag, ndocs, vocab, queries, sparse=(7, 5), seed=12345, with_slots=True):
     """Xapiand's own multivalue classes (oracle/_ref/libxapiand_mv_ref.so = src/multivalue/range.cc, keymaker.cc …
     compiled from the reference): slots written as StringLists of Serialise::positive keys, MultipleValueRange as
-    OP_FILTER right side or weighted OP_AND child, Multi_MultiValueKeyMaker{SerialiseKey} as the sorter."""
+    OP_FILTER right side or weighted OP_AND child, Multi_MultiValueKeyMaker{SerialiseKey} as the sorter.
+    with_slots records the slot bytes too (multivalue_5k's are what the device test builds its index from)."""
     import subprocess
     tmp = tempfile.mkdtemp(prefix="xgm_golden_")
     try:
         d = os.path.join(tmp, "db")
         O.ref_build(d, ndocs, vocab, seed=seed, mvalues=True, sparse=sparse)
-        lines = [O.query_line("TERM" if len(q["terms"]) == 1 else "AND", [name(t) for t in q["terms"]], q["first"],
+        lines = [O.query_line("TERM" if len(q["terms"]) == 1 else q.get("op", "AND"), [name(t) for t in q["terms"]], q["first"],
                               q["maxitems"], q["check_at_least"], mvr=q.get("mvr"), keysort=q.get("keysort"))
                  for q in queries]
         info, res = O.ref_query([d], lines, os.path.join(tmp, "w"))
         slots = {}
-        for ln in subprocess.check_output([O.REF_RUNNER, "slots", "--db", d]).decode().splitlines():
+        for ln in subprocess.check_output([O.REF_RUNNER, "slots", "--db", d]).decode().splitlines() if with_slots else ():
             sl, did, hx = (ln.split() + [""])[:3]
             slots.setdefault(sl, {})[did] = hx
         nums = sorted({v for q in queries if q.get("mvr") for v in q["mvr"][1:3]})
         ser = subprocess.check_output([O.REF_RUNNER, "serialise"] + [str(v) for v in nums]).decode().split()
-        fixture = dict(tag=tag, ndocs=ndocs, vocab=vocab, seed=seed, sparse=list(sparse), slots=slots,
+        fixture = dict(tag=tag, ndocs=ndocs, vocab=vocab, seed=seed, sparse=list(sparse),
                        serialised=dict(zip(map(str, nums), ser)), queries=[])
+        if with_slots:
+            fixture["slots"] = slots
         for q, r in zip(queries, res):
             e = dict(q)
             e["docids"] = r.docids
@@ -113,6 +116,50 @@ def mv_queries(rng, n, topranks, ndocs):
             q["mvr"] = [0, lo, lo + rng.choice([5000, 50000, 300000]), 1 if kind == 2 else 0]
         if i % 3 != 1:
             q["keysort"] = [rng.choice([0, 1, 1]), rng.choice([0, 1])]
+        qs.append(q)
+    return qs
+
+
+def orvalues_queries(rng, n, ndocs, past_end):
+    """OP_FILTER(base, MultipleValueRange) on OR bases of 2..5 leaves (the or3 kernel) and of 6..16 (the general OR
+    kernel), with a single term and a two-term AND as controls; ranges matching nothing, narrow, wide and covering
+    every value; no sort or KEYSORT forward / reverse; `first` past_end is beyond every filtered match count."""
+    qs = []
+    for i in range(n):
+        base, kind = i % 4, (i // 4) % 4
+        if base == 0:
+            op, terms = "OR", rng.sample(range(40), rng.randint(2, 5))
+        elif base == 1:
+            op, terms = "OR", rng.sample(range(60), rng.randint(6, 16))
+        else:
+            op, terms = "AND", rng.sample(range(20), base - 1)
+        lo = rng.randrange(0, 950000)
+        lo, hi = ((2000000, 3000000), (lo, lo + 5000), (lo, lo + 400000), (0, 1000000))[kind]
+        q = dict(op=op, terms=terms, first=rng.choice([0, 0, 3, past_end]),
+                 maxitems=rng.choice([0, 1, 1, 10, 10, 100]), check_at_least=rng.choice([0, 200, ndocs]),
+                 mvr=[0, lo, hi, 0])
+        if rng.random() < 0.6:
+            q["keysort"] = [rng.choice([0, 1]), rng.choice([0, 1])]
+        qs.append(q)
+    return qs
+
+
+def vrbounds_queries(rng, n, ndocs):
+    """OP_FILTER(base, OP_VALUE_RANGE) on a slot every document has, over ANDs of frequent terms and OR bases: ranges
+    covering every value (the range's termfreq min is value_freq) or part of them (min 0)."""
+    qs = []
+    for i in range(n):
+        base, kind = i % 3, (i // 3) % 3
+        if base == 0:
+            op, terms = "AND", rng.sample(range(15), rng.choice([1, 2]))
+        else:
+            op, terms = "OR", rng.sample(range(60), rng.randint(2, 5) if base == 1 else rng.randint(6, 12))
+        lo = rng.randrange(0, 900000)
+        lo, hi = ((0, 1000000), (lo, lo + 10000), (lo, lo + 400000))[kind]
+        q = dict(op=op, terms=terms, first=rng.choice([0, 0, 3]), maxitems=rng.choice([0, 1, 1, 10, 10, 100]),
+                 check_at_least=rng.choice([0, 200, ndocs]), vr=[0, lo, hi])
+        if i % 2:
+            q["sort"] = [1, rng.choice([0, 1])]
         qs.append(q)
     return qs
 
@@ -242,6 +289,9 @@ def main():
     if sys.argv[1:] == ["orops"]:
         run_set("orops_6k", 6000, 900, orops_queries(random.Random(20260931), 240, 120, 6000), seed=11)
         return
+    if sys.argv[1:] == ["ranges"]:
+        range_sets()
+        return
     if sys.argv[1:] == ["ops"]:  # only the fixtures added after round 1's first batch
         run_set("ops_6k", 6000, 900, ops_queries(random.Random(20260924), 240, 200, 6000), seed=11)
         run_set("scale_6k", 6000, 900, scale_queries(random.Random(20260925), 200, 200, 6000), seed=11)
@@ -283,6 +333,17 @@ def main():
     run_set("bm25_6k", 6000, 900, bm25_queries(random.Random(20260929), 200, 150, 6000), seed=11)
     run_mv_set("multivalue_5k", 5000, 2000, mv_queries(random.Random(20260930), 240, 60, 5000))
     run_set("orops_6k", 6000, 900, orops_queries(random.Random(20260931), 240, 120, 6000), seed=11)
+    range_sets()
+
+
+def range_sets():
+    """Value-range filters over OR bases: Xapiand slots with the sparse rule of multivalue_5k (value_freq 4279) and a
+    much sparser one (about half the documents), so that value_freq falls well below an OR's termfreq max; and
+    stock OP_VALUE_RANGE."""
+    run_mv_set("orvalues_5k", 5000, 2000, orvalues_queries(random.Random(20261017), 48, 5000, 4500), with_slots=False)
+    run_mv_set("orvalues_sparse_5k", 5000, 2000, orvalues_queries(random.Random(20261018), 48, 5000, 4500),
+               sparse=(2, 5), with_slots=False)
+    run_set("vrbounds_5k", 5000, 2000, vrbounds_queries(random.Random(20261019), 27, 5000), values=True)
 
 
 if __name__ == "__main__":

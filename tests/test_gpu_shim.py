@@ -20,7 +20,7 @@ pytestmark = [pytest.mark.gpu,
 #            fixture           min. share of queries libxgm must answer itself
 FIXTURES = [("c1_1k_100", 0.95), ("mid_20k", 0.95), ("ops_6k", 0.9), ("orops_6k", 0.5), ("scale_6k", 0.7), ("regimes_6k", 0.9),
             ("wqf_6k", 0.95), ("sortmodes_6k", 0.9), ("bm25_6k", 0.8), ("values_5k", 0.95), ("multivalue_5k", 0.95),
-            ("shard4_20k", 0.95)]
+            ("shard4_20k", 0.95), ("orvalues_5k", 0.6), ("orvalues_sparse_5k", 0.6), ("vrbounds_5k", 0.95)]
 
 
 @pytest.mark.parametrize("tag,min_served", FIXTURES)

@@ -180,7 +180,8 @@ def test_round_estimate_examples():
 
 def mv_o_query(q):
     """multivalue_5k fixture → oracle query: Xapiand's MultipleValueRange / Multi_MultiValueKeyMaker shapes."""
-    kw = dict(op=O.OP_AND, terms=q["terms"], first=q["first"], maxitems=q["maxitems"], check_at_least=q["check_at_least"])
+    kw = dict(op=O.OP_OR if q.get("op") == "OR" else O.OP_AND, terms=q["terms"], first=q["first"],
+              maxitems=q["maxitems"], check_at_least=q["check_at_least"])
     if "mvr" in q:
         kw.update(filter=O.FILTER_MULTI_RANGE, range_lo=q["mvr"][1], range_hi=q["mvr"][2], filter_weighted=bool(q["mvr"][3]))
     if "keysort" in q:
@@ -204,12 +205,66 @@ def test_oracle_matches_xapiand_multivalue_classes():
         m = ix.match(mv_o_query(q))
         check(m, q, f"mv[{i}] {q['terms']} mvr={q.get('mvr')} keysort={q.get('keysort')}")
         kinds.add((q.get("mvr", [0, 0, 0, -1])[3], tuple(q.get("keysort", ()))))
-        if "keysort" in q:  # same order relation between consecutive sort keys (byte strings vs the oracle's scale)
-            keys = [bytes.fromhex(k) for k in q.get("sort_keys", [])]
-            mine = list(m.sortvals)
-            rev = bool(q["keysort"][1])
-            for a in range(len(keys) - 1):
-                # reverse keys are complemented: ascending bytes = descending values
-                assert (keys[a] < keys[a + 1]) == ((mine[a] > mine[a + 1]) if rev else (mine[a] < mine[a + 1])), i
-                assert (keys[a] == keys[a + 1]) == (mine[a] == mine[a + 1]), i
+        check_keysort_order(m, q, i)
     assert len(kinds) >= 10
+
+
+def check_keysort_order(m, q, ctx):
+    """Same order relation between consecutive sort keys (byte strings vs the oracle's scale)."""
+    if "keysort" not in q:
+        return
+    keys = [bytes.fromhex(k) for k in q.get("sort_keys", [])]
+    mine = list(m.sortvals)
+    rev = bool(q["keysort"][1])
+    for a in range(len(keys) - 1):
+        # reverse keys are complemented: ascending bytes = descending values
+        assert (keys[a] < keys[a + 1]) == ((mine[a] > mine[a + 1]) if rev else (mine[a] < mine[a + 1])), ctx
+        assert (keys[a] == keys[a + 1]) == (mine[a] == mine[a + 1]), ctx
+
+
+def range_kind(lo, hi):
+    return "nothing" if lo >= 2000000 else "all" if (lo, hi) == (0, 1000000) else "narrow" if hi - lo <= 10000 else "wide"
+
+
+@pytest.mark.parametrize("tag", ["orvalues_5k", "orvalues_sparse_5k"])
+def test_oracle_matches_reference_range_source_on_or_bases(tag):
+    """OP_FILTER(base, MultipleValueRange) on OR bases of 2..5 and 6..16 leaves, single terms and ANDs: the reference
+    runs it as a MultiAndPostList of [base, source] whose termfreqs fold in the source's (0, value_freq, value_freq)
+    (range.cc:457-464), so the upper bound is at most value_freq and the lower bound is usually 0.  Docids, weights,
+    sort keys, percentages and all three bounds bit-equal with the compiled reference."""
+    fx = load(tag)
+    ix = O.Index.synthetic(fx["ndocs"], fx["vocab"], fx["seed"], values=True)
+    ix.make_sparse(*fx["sparse"])
+    vf = int((ix.values()[0] != 0).sum())
+    shapes, clipped = set(), 0
+    for i, q in enumerate(fx["queries"]):
+        m = ix.match(mv_o_query(q))
+        ctx = f"{tag}[{i}] {q['op']} {q['terms']} mvr={q['mvr']} keysort={q.get('keysort')}"
+        check(m, q, ctx)
+        check_keysort_order(m, q, ctx)
+        base = "single" if len(q["terms"]) == 1 else q["op"] + ("-wide" if len(q["terms"]) > 5 else "")
+        shapes.add((base, range_kind(*q["mvr"][1:3])))
+        if q["op"] == "OR":  # the reference's bound lies below the OR tree's own
+            whole = ix.match(O.Query(op=O.OP_OR, terms=q["terms"], maxitems=0))
+            clipped += q["ub"] == vf < whole.ub
+    assert len(shapes) == 16, sorted(shapes)
+    assert clipped >= 3, clipped
+
+
+def test_oracle_matches_reference_value_range_bounds():
+    """Stock OP_VALUE_RANGE on AND and OR bases: the range's termfreq max is value_freq and its min value_freq when it
+    covers the slot's value bounds, 0 otherwise (valuerangepostlist.cc:40-54,145-148), so the lower and upper
+    bounds are exact; the estimate folds in the range's string-fraction estimate, which is not restated.  A range
+    covering every value of a slot all documents have is the all-documents list: no matching subquery for the
+    percentages."""
+    fx = load("vrbounds_5k")
+    ix = O.Index.synthetic(fx["ndocs"], fx["vocab"], fx["seed"], values=True)
+    covering = 0
+    for i, q in enumerate(fx["queries"]):
+        m = ix.match(o_query(q))
+        ctx = f"vrbounds[{i}] {q}"
+        check(m, q, ctx, counts=False)
+        assert bits(m.max_possible) == bits(q["max_possible"]), f"{ctx}: max_possible"
+        assert (m.lb, m.ub) == (q["lb"], q["ub"]), f"{ctx}: bounds"
+        covering += q["vr"][1:] == [0, 1000000] and q["lb"] > 0
+    assert covering >= 5, covering

@@ -135,6 +135,10 @@ struct xgm_index {
     uint64_t slot_max[XGM_MAX_SLOTS] = {};
     uint64_t slot_min[XGM_MAX_SLOTS] = {};
     uint32_t slot_freq[XGM_MAX_SLOTS] = {}; /* documents with a value in the slot (Database::get_value_freq) */
+    /* least and greatest first value of a document: the slot's value bounds as a stock value range, which reads
+     * the first value, sees them (Database::get_value_lower_bound / get_value_upper_bound) */
+    uint64_t slot_first_min[XGM_MAX_SLOTS] = {};
+    uint64_t slot_first_max[XGM_MAX_SLOTS] = {};
     bool slot_exact[XGM_MAX_SLOTS] = {};
     int sm_count = 132; /* H100 SXM; replaced by the device's count at upload */
     /* Large batches fill the GPU on their own: the kernels of all searchers of this index go through one
@@ -339,7 +343,14 @@ static xgm_status upload_index(xgm_index* ix, std::vector<Chunk>& chunks, const 
             CUDA_TRY(cudaMemcpy(ix->d_vals[s], slots[s].vals.data(), slots[s].vals.size() * 8, cudaMemcpyHostToDevice));
         ix->slot_min[s] = slots[s].vals.empty() ? 0 : ~0ull;
         for (uint64_t v : slots[s].vals) { ix->slot_max[s] = std::max(ix->slot_max[s], v); ix->slot_min[s] = std::min(ix->slot_min[s], v); }
-        for (size_t d = 0; d + 1 < slots[s].voff.size(); ++d) ix->slot_freq[s] += slots[s].voff[d + 1] > slots[s].voff[d];
+        ix->slot_first_min[s] = slots[s].vals.empty() ? 0 : ~0ull;
+        for (size_t d = 0; d + 1 < slots[s].voff.size(); ++d) {
+            if (slots[s].voff[d + 1] == slots[s].voff[d]) continue;
+            const uint64_t v = slots[s].vals[slots[s].voff[d]];
+            ++ix->slot_freq[s];
+            ix->slot_first_min[s] = std::min(ix->slot_first_min[s], v);
+            ix->slot_first_max[s] = std::max(ix->slot_first_max[s], v);
+        }
         ix->slot_exact[s] = slots[s].exact;
     }
     ix->nblocks = 0;
@@ -919,8 +930,9 @@ struct PlannedQuery {
     uint64_t alg_bytes = 0;
     uint32_t sort_by = 0;
     uint32_t filter = 0;
+    bool filter_subq = false; /* the filter counts as a matching subquery of every match */
     double bucket_max = 0;   /* finite bound of the weights, for the pruning buckets (max_possible is DBL_MAX with a weighted source) */
-    bool mv_source = false;  /* a Xapiand range source is a child of the AND: its termfreq estimates are restated */
+    bool mv_source = false;  /* a Xapiand range source is a child of the base's MultiAndPostList: its termfreqs are restated */
     bool count_only = false; /* first >= every possible match count: the MSet is empty, only counts matter */
     bool aux_subqs = false;  /* the number of matching weighted leaves varies per document (OR, AND_MAYBE) */
     bool log_raises = false; /* … and the MSet is not ordered by weight: subqueries of the best-weighted document come from the raise log */
@@ -1508,22 +1520,38 @@ static TfNode group_bounds(const xgm_index* ix, const PlanTerms& t, TfNode cur) 
  * which the bitmap AND kernel tests the coarse bit first (DESIGN.md §6: chosen by measurement on C2 and C5). */
 #define XGM_COARSE_PASS_MAX 0.1
 
-/* An AND base: one MultiAndPostList over the base terms and, for a Xapiand range, its source; the FILTER terms join
+/* The range of OP_FILTER(base, range) as a MultiAndPostList child.  The source of a Xapiand range
+ * (MultipleValueRange) has termfreqs (min, est, max) = (0, value_freq, value_freq) (range.cc:457-464,
+ * api/postingsource.cc:201-214).  A stock OP_VALUE_RANGE has max = value_freq and min = value_freq when the range
+ * covers the slot's value bounds, 0 otherwise (valuerangepostlist.cc:40-54,145-148); its string-fraction estimate
+ * (valuerangepostlist.cc:70-130) is not restated: value_freq stands in for it and finish_info flags the bounds. */
+static bool stock_range_covers_slot(const xgm_index* ix, const xgm_query& q) {
+    const uint32_t s = q.filter_slot;
+    return q.filter == XGM_FILTER_VALUE_RANGE && ix->slot_freq[s] != 0 && q.range_lo <= ix->slot_first_min[s] &&
+           ix->slot_first_max[s] <= q.range_hi;
+}
+
+static TfNode range_child(const xgm_index* ix, const xgm_query& q) {
+    const uint32_t vf = ix->slot_freq[q.filter_slot];
+    return TfNode{stock_range_covers_slot(ix, q) ? vf : 0u, vf, vf};
+}
+
+/* An AND base: one MultiAndPostList over the base terms and, for a value range, the range; the FILTER terms join
  * the required lists as boolean leaves, then the AND_NOT and AND_MAYBE terms follow. */
 static void plan_and_route(const xgm_index* ix, const xgm_query& q, const PlanTerms& t, PlannedQuery& pq,
                            XgmDevQuery& dq) {
     const uint32_t n = t.n;
-    /* the source of a Xapiand range (MultipleValueRange) takes part in the MultiAndPostList like a term with
-     * termfreq (min, est, max) = (0, value_freq, value_freq) (range.cc:457-464, api/postingsource.cc:201-214) */
+    /* the range takes part in the MultiAndPostList like a term (a weighted one only as a Xapiand range's source) */
+    const bool has_range = q.filter != XGM_FILTER_NONE;
     const bool mv_source = q.filter == XGM_FILTER_MULTI_RANGE;
     const bool src_weighted = mv_source && q.filter_weighted;
     const double src_w = src_weighted ? (q.filter_factor != 0.0 ? q.filter_factor : 1.0) : 0.0;
     /* its children sorted by get_termfreq_est with the very call of multiandpostlist.h:126-131 */
-    const uint32_t nch = n + (mv_source ? 1u : 0u);
-    const uint32_t src_vf = mv_source ? ix->slot_freq[q.filter_slot] : 0u;
+    const uint32_t nch = n + (has_range ? 1u : 0u);
+    const TfNode src = has_range ? range_child(ix, q) : TfNode{0, 0, 0};
     TfIdx in[XGM_MAX_TERMS + 1], outv[XGM_MAX_TERMS + 1];
     for (uint32_t j = 0; j < n; ++j) in[j] = TfIdx{t.ltf[j], j};
-    if (mv_source) in[n] = TfIdx{src_vf, n};
+    if (has_range) in[n] = TfIdx{src.est, n};
     std::partial_sort_copy(in, in + nch, outv, outv + nch, tf_less);
     /* MultiAndPostList::recalc_maxweight (multiandpostlist.cc:167-177) and termfreqs over the children in that
      * order: base term order[i], or the source at src_pos */
@@ -1534,7 +1562,7 @@ static void plan_and_route(const xgm_index* ix, const xgm_query& q, const PlanTe
         const uint32_t j = outv[c].idx;
         if (j == n) {
             src_pos = k;
-            ch[c] = TfNode{0, src_vf, src_vf};
+            ch[c] = src;
             mp += src_weighted ? src_w * DBL_MAX : 0.0;
             mp_real += src_w;
         } else {
@@ -1592,7 +1620,8 @@ static void plan_and_route(const xgm_index* ix, const xgm_query& q, const PlanTe
 /* An OR base of several leaves: a Huffman-shaped tree of binary OrPostLists, built from the leaves in query order
  * (OrContext::postlist, queryinternal.cc:440-489).  On the device the leaves are stored in ascending-termfreq order
  * (position = ownership priority); the program refers to positions. */
-static void plan_or_route(const xgm_index* ix, const PlanTerms& t, PlannedQuery& pq, XgmDevQuery& dq) {
+static void plan_or_route(const xgm_index* ix, const xgm_query& q, const PlanTerms& t, PlannedQuery& pq,
+                          XgmDevQuery& dq) {
     const uint32_t n = t.n;
     TfIdx in[XGM_MAX_TERMS];
     for (uint32_t j = 0; j < n; ++j) in[j] = TfIdx{t.ltf[j], j};
@@ -1600,11 +1629,20 @@ static void plan_or_route(const xgm_index* ix, const PlanTerms& t, PlannedQuery&
     uint32_t posof[XGM_MAX_TERMS];
     for (uint32_t i = 0; i < n; ++i) posof[in[i].idx] = i;
     const OrFold f = or_fold(t.ltf, t.maxpart, n, ix->doccount, posof, &dq);
-    /* QueryFilter / QueryAndNot above the OrPostList tree: the filter's boolean terms and the excluded terms weigh
-     * nothing (MultiAndPostList::get_weight adds +0.0, AndNotPostList returns the left's weight), so a match keeps
-     * the tree's weight; the counts follow the same bound arithmetic as around an AND base. */
-    const TfNode cur = group_bounds(ix, t, f.tf);
+    /* QueryFilter / QueryAndNot above the OrPostList tree: the filter's boolean terms, a value range and the excluded
+     * terms weigh nothing (MultiAndPostList::get_weight adds +0.0, AndNotPostList returns the left's weight), so a
+     * match keeps the tree's weight; the counts follow the same bound arithmetic as around an AND base.  A value
+     * range comes without groups: QueryFilter::postlist's MultiAndPostList of [tree, range] (queryinternal.cc:
+     * 2271-2283), its two children by ascending estimate. */
+    TfNode cur = f.tf;
+    if (q.filter != XGM_FILTER_NONE) {
+        const TfNode src = range_child(ix, q);
+        const TfNode ch[2] = {src.est < cur.est ? src : cur, src.est < cur.est ? cur : src};
+        cur = and_node(ch, 2, ix->doccount);
+    }
+    cur = group_bounds(ix, t, cur);
     pq.tf_min = cur.mn; pq.tf_max = cur.mx; pq.tf_est = cur.est;
+    pq.mv_source = q.filter == XGM_FILTER_MULTI_RANGE;
     pq.max_possible = f.maxw;
     pq.bucket_max = pq.max_possible;
     pq.nweighted = t.nweighted; /* every leaf: a zero factor was declined */
@@ -1637,6 +1675,10 @@ static void plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, Planned
     cal = std::max(cal, first + maxitems);
     pq.first = first; pq.maxitems = maxitems; pq.topk = first + maxitems; pq.check_at_least = cal;
     pq.sort_by = q.sort_by; pq.filter = q.filter;
+    /* a stock range covering every value of a slot that every document has is matched by the all-documents list
+     * (QueryValueRange::postlist, queryinternal.cc:1116-1124), an unweighted leaf: no matching subquery */
+    pq.filter_subq = q.filter != XGM_FILTER_NONE &&
+                     !(stock_range_covers_slot(ix, q) && ix->slot_freq[q.filter_slot] == ix->doccount);
     pq.status = weigh_terms(ix, q, t);
     if (pq.status != XGM_OK) return;
 
@@ -1648,7 +1690,7 @@ static void plan_query(xgm_searcher* s, const xgm_query& q, uint32_t qi, Planned
     dq.sort_missing = q.sort_missing_key;
     dq.src_pos = XGM_NO_SRC; dq.src_weight = 0.0;
     if (q.op == XGM_OP_AND || t.n == 1) plan_and_route(ix, q, t, pq, dq);
-    else plan_or_route(ix, t, pq, dq);
+    else plan_or_route(ix, q, t, pq, dq);
 
     /* algorithmic bytes, SURVEY.md §8(d): compressed columns + 16 B per block header of every query
      * term (full lists, no credit for skipping) + 16 B per result; 4 B per candidate added at wait() */
@@ -2049,11 +2091,13 @@ static void finish_info(const PlannedQuery& pq, const XgmDevResult* dr, const ui
         /* a count-only query keeps one document only for the percentage scale: its bounds are the exact count */
         if ((dr->flags & XGM_RES_APPROX) && !pq.count_only) o->flags |= XGM_MSET_BOUNDS_APPROX;
         if (dr->flags & XGM_RES_SKIPPED) o->flags |= XGM_MSET_BOUNDS_APPROX | XGM_MSET_COUNT_LOWER_BOUND;
-        /* with a value-range source in the AND the reference's lower bound / estimate also fold in
-         * ValueRangePostList::get_termfreq_est (valuerangepostlist.cc:70-130), which is not restated */
+        /* with a stock value range the reference's estimate folds in ValueRangePostList::get_termfreq_est
+         * (valuerangepostlist.cc:70-130), which is not restated (range_child) */
         if (pq.filter && !pq.mv_source && size == pq.topk && known >= pq.check_at_least) o->flags |= XGM_MSET_BOUNDS_APPROX;
     } else if (pq.check_at_least != 0) {
         lb = est = ub = 0; /* empty result set: !full() branch */
+    } else if (pq.filter && !pq.mv_source) {
+        o->flags |= XGM_MSET_BOUNDS_APPROX; /* bounds only, with a stock value range's estimate as above */
     }
     o->matches_lower_bound = o->uncollapsed_lower_bound = lb;
     o->matches_estimated = o->uncollapsed_estimated = est;
@@ -2079,7 +2123,7 @@ static void finish_info(const PlannedQuery& pq, const XgmDevResult* dr, const ui
         /* a value-range / posting-source filter counts as a matching subquery (ValueRangePostList /
          * ExternalPostList::count_matching_subqs return 1) without being one of the total weighted leaves
          * (api/queryinternal.cc:1097-1098) */
-        if (pq.filter) subqs += 1;
+        if (pq.filter_subq) subqs += 1;
         double percent_scale = (double)subqs / (double)pq.nweighted;
         percent_scale /= max_w;
         o->percent_scale_factor = percent_scale * 100.0;
