@@ -91,6 +91,60 @@ static int default_threads() {
 
 static inline uint32_t bits_for(uint32_t v) { return v ? 32u - (uint32_t)__builtin_clz(v) : 0u; }
 
+/* ------------------------------------------------------------------ owned CUDA resources */
+
+/* A device (cudaMalloc) or pinned host (cudaMallocHost) array of T that frees itself.  The destructor and every
+ * reallocation free on the current device: whoever frees one sets it first. */
+template <class T, bool Pinned> class Buf {
+  public:
+    Buf() = default;
+    Buf(const Buf&) = delete;
+    Buf& operator=(const Buf&) = delete;
+    ~Buf() { release(); }
+    /* n elements; what was held before is freed first */
+    cudaError_t alloc(size_t n) {
+        release();
+        void* p = nullptr;
+        const cudaError_t e = Pinned ? cudaMallocHost(&p, n * sizeof(T)) : cudaMalloc(&p, n * sizeof(T));
+        if (e == cudaSuccess) { p_ = static_cast<T*>(p); cap_ = n; }
+        return e;
+    }
+    /* room for `need` elements, grown to max(2 need, floor); the stream's copies and kernels may still read the
+     * old array, so it is waited for before the array is freed */
+    cudaError_t grow(size_t need, size_t floor, cudaStream_t st) {
+        if (need <= cap_) return cudaSuccess;
+        const cudaError_t e = cudaStreamSynchronize(st);
+        return e != cudaSuccess ? e : alloc(std::max(need * 2, floor));
+    }
+    T* get() const { return p_; }
+
+  private:
+    void release() {
+        if (p_) { if (Pinned) cudaFreeHost(p_); else cudaFree(p_); }
+        p_ = nullptr; cap_ = 0;
+    }
+    T* p_ = nullptr;
+    size_t cap_ = 0;
+};
+template <class T> using DevBuf = Buf<T, false>;
+template <class T> using HostBuf = Buf<T, true>;
+
+/* A CUDA event or stream that is destroyed with its owner */
+template <class H, cudaError_t (*Create)(H*, unsigned int), cudaError_t (*Destroy)(H)> class Handle {
+  public:
+    Handle() = default;
+    Handle(const Handle&) = delete;
+    Handle& operator=(const Handle&) = delete;
+    ~Handle() { if (h_) Destroy(h_); }
+    cudaError_t create(unsigned int flags) { return Create(&h_, flags); }
+    H get() const { return h_; }
+
+  private:
+    H h_ = nullptr;
+};
+using Event = Handle<cudaEvent_t, cudaEventCreateWithFlags, cudaEventDestroy>;
+using Stream = Handle<cudaStream_t, cudaStreamCreateWithFlags, cudaStreamDestroy>;
+
 /* ------------------------------------------------------------------ index */
 
 struct TermInfo {
@@ -122,16 +176,21 @@ struct xgm_index {
     std::vector<TermInfo> terms;
     std::unordered_map<std::string, uint32_t> dict;
     bool synthetic_names = false; /* "T%06u" names resolved arithmetically, no dictionary */
+    /* Large batches fill the GPU on their own: the kernels of all searchers of this index go through one
+     * FIFO compute stream (copies stay on the searchers' streams), so that batch k's results are not
+     * delayed by batch k+1's kernels sharing the SMs with them.  Declared before the arrays: destroyed after them. */
+    mutable Stream compute_stream;
+    mutable std::mutex launch_mu;
     /* device */
-    XgmBlockHdr* d_hdr = nullptr;
-    uint4* d_docs = nullptr;
-    uint4* d_tfs = nullptr;
-    uint32_t* d_doclen = nullptr;
-    uint32_t* d_bitmaps = nullptr;
-    uint32_t* d_coarse = nullptr; /* a bit per 8 docids of d_bitmaps (xgm_format.h) */
-    uint32_t* d_ranks = nullptr;
-    uint32_t* d_voff[XGM_MAX_SLOTS] = {};
-    uint64_t* d_vals[XGM_MAX_SLOTS] = {};
+    DevBuf<XgmBlockHdr> d_hdr;
+    DevBuf<uint32_t> d_docs; /* the kernels read it as uint4 */
+    DevBuf<uint32_t> d_tfs;
+    DevBuf<uint32_t> d_doclen;
+    DevBuf<uint32_t> d_bitmaps;
+    DevBuf<uint32_t> d_coarse; /* a bit per 8 docids of d_bitmaps (xgm_format.h) */
+    DevBuf<uint32_t> d_ranks;
+    DevBuf<uint32_t> d_voff[XGM_MAX_SLOTS];
+    DevBuf<uint64_t> d_vals[XGM_MAX_SLOTS];
     uint64_t slot_max[XGM_MAX_SLOTS] = {};
     uint64_t slot_min[XGM_MAX_SLOTS] = {};
     uint32_t slot_freq[XGM_MAX_SLOTS] = {}; /* documents with a value in the slot (Database::get_value_freq) */
@@ -141,11 +200,8 @@ struct xgm_index {
     uint64_t slot_first_max[XGM_MAX_SLOTS] = {};
     bool slot_exact[XGM_MAX_SLOTS] = {};
     int sm_count = 132; /* H100 SXM; replaced by the device's count at upload */
-    /* Large batches fill the GPU on their own: the kernels of all searchers of this index go through one
-     * FIFO compute stream (copies stay on the searchers' streams), so that batch k's results are not
-     * delayed by batch k+1's kernels sharing the SMs with them. */
-    mutable cudaStream_t compute_stream = nullptr;
-    mutable std::mutex launch_mu;
+    /* the members free their arrays and stream on the index's device, also when a build failed half-way */
+    ~xgm_index() { cudaSetDevice(device); }
 };
 
 /* Compressed form of a contiguous range of terms, produced by one builder thread. */
@@ -293,13 +349,13 @@ static xgm_status upload_index(xgm_index* ix, std::vector<Chunk>& chunks, const 
             if (ix->terms[t].bm_off != XGM_NO_BITMAP) { ix->terms[t].bm_off += bmb[i]; ix->terms[t].rk_off += rkb[i]; }
         }
     });
-    CUDA_TRY(cudaMalloc(&ix->d_bitmaps, std::max<size_t>(nbm, 8) * 4));
-    CUDA_TRY(cudaMalloc(&ix->d_ranks, std::max<size_t>(nrk, 8) * 4));
+    CUDA_TRY(ix->d_bitmaps.alloc(std::max<size_t>(nbm, 8)));
+    CUDA_TRY(ix->d_ranks.alloc(std::max<size_t>(nrk, 8)));
     for (size_t i = 0; i < chunks.size(); ++i) {
         if (!chunks[i].bitmaps.empty())
-            CUDA_TRY(cudaMemcpy(ix->d_bitmaps + bmb[i], chunks[i].bitmaps.data(), chunks[i].bitmaps.size() * 4, cudaMemcpyHostToDevice));
+            CUDA_TRY(cudaMemcpy(ix->d_bitmaps.get() + bmb[i], chunks[i].bitmaps.data(), chunks[i].bitmaps.size() * 4, cudaMemcpyHostToDevice));
         if (!chunks[i].ranks.empty())
-            CUDA_TRY(cudaMemcpy(ix->d_ranks + rkb[i], chunks[i].ranks.data(), chunks[i].ranks.size() * 4, cudaMemcpyHostToDevice));
+            CUDA_TRY(cudaMemcpy(ix->d_ranks.get() + rkb[i], chunks[i].ranks.data(), chunks[i].ranks.size() * 4, cudaMemcpyHostToDevice));
         std::vector<uint32_t>().swap(chunks[i].bitmaps);
         std::vector<uint32_t>().swap(chunks[i].ranks);
     }
@@ -308,39 +364,39 @@ static xgm_status upload_index(xgm_index* ix, std::vector<Chunk>& chunks, const 
         if (t.bm_off != XGM_NO_BITMAP && (t.bm_off & 7u) != 0)
             return fail(XGM_E_INVALID, "membership bitmap offset %llu is not a multiple of 8 words", (unsigned long long)t.bm_off);
     const size_t ncoarse = nbm / 8;
-    CUDA_TRY(cudaMalloc(&ix->d_coarse, std::max<size_t>(ncoarse, 8) * 4));
-    CUDA_TRY(xgm_launch_coarse(ix->d_bitmaps, ncoarse, ix->d_coarse, 0));
+    CUDA_TRY(ix->d_coarse.alloc(std::max<size_t>(ncoarse, 8)));
+    CUDA_TRY(xgm_launch_coarse(ix->d_bitmaps.get(), ncoarse, ix->d_coarse.get(), 0));
     CUDA_TRY(cudaDeviceSynchronize());
     ix->bytes_bitmaps = (nbm + ncoarse + nrk) * 4;
     /* +16 bytes slack at the end of each column: the unpackers may read one word past a block */
-    CUDA_TRY(cudaMalloc(&ix->d_hdr, (nh + 1) * sizeof(XgmBlockHdr)));
-    CUDA_TRY(cudaMalloc(&ix->d_docs, nd * 4 + 64));
-    CUDA_TRY(cudaMalloc(&ix->d_tfs, nt * 4 + 64));
-    CUDA_TRY(cudaMemset(reinterpret_cast<char*>(ix->d_docs) + nd * 4, 0, 64));
-    CUDA_TRY(cudaMemset(reinterpret_cast<char*>(ix->d_tfs) + nt * 4, 0, 64));
+    CUDA_TRY(ix->d_hdr.alloc(nh + 1));
+    CUDA_TRY(ix->d_docs.alloc(nd + 16));
+    CUDA_TRY(ix->d_tfs.alloc(nt + 16));
+    CUDA_TRY(cudaMemset(ix->d_docs.get() + nd, 0, 64));
+    CUDA_TRY(cudaMemset(ix->d_tfs.get() + nt, 0, 64));
     for (size_t i = 0; i < chunks.size(); ++i) {
         if (!chunks[i].hdr.empty())
-            CUDA_TRY(cudaMemcpy(ix->d_hdr + hb[i], chunks[i].hdr.data(), chunks[i].hdr.size() * sizeof(XgmBlockHdr), cudaMemcpyHostToDevice));
+            CUDA_TRY(cudaMemcpy(ix->d_hdr.get() + hb[i], chunks[i].hdr.data(), chunks[i].hdr.size() * sizeof(XgmBlockHdr), cudaMemcpyHostToDevice));
         if (!chunks[i].docs.empty())
-            CUDA_TRY(cudaMemcpy(reinterpret_cast<uint32_t*>(ix->d_docs) + dbase[i], chunks[i].docs.data(), chunks[i].docs.size() * 4, cudaMemcpyHostToDevice));
+            CUDA_TRY(cudaMemcpy(ix->d_docs.get() + dbase[i], chunks[i].docs.data(), chunks[i].docs.size() * 4, cudaMemcpyHostToDevice));
         if (!chunks[i].tfs.empty())
-            CUDA_TRY(cudaMemcpy(reinterpret_cast<uint32_t*>(ix->d_tfs) + tb[i], chunks[i].tfs.data(), chunks[i].tfs.size() * 4, cudaMemcpyHostToDevice));
+            CUDA_TRY(cudaMemcpy(ix->d_tfs.get() + tb[i], chunks[i].tfs.data(), chunks[i].tfs.size() * 4, cudaMemcpyHostToDevice));
         std::vector<XgmBlockHdr>().swap(chunks[i].hdr);
         std::vector<uint32_t>().swap(chunks[i].docs);
         std::vector<uint32_t>().swap(chunks[i].tfs);
     }
     XgmBlockHdr tail;
     tail.first = XGM_SENTINEL; tail.doc_off = 0; tail.tf_off = 0; tail.meta = 0;
-    CUDA_TRY(cudaMemcpy(ix->d_hdr + nh, &tail, sizeof(tail), cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMalloc(&ix->d_doclen, doclen.size() * 4));
-    CUDA_TRY(cudaMemcpy(ix->d_doclen, doclen.data(), doclen.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(ix->d_hdr.get() + nh, &tail, sizeof(tail), cudaMemcpyHostToDevice));
+    CUDA_TRY(ix->d_doclen.alloc(doclen.size()));
+    CUDA_TRY(cudaMemcpy(ix->d_doclen.get(), doclen.data(), doclen.size() * 4, cudaMemcpyHostToDevice));
     for (int s = 0; s < XGM_MAX_SLOTS; ++s) {
         if (!slots || !slots[s].present) continue;
-        CUDA_TRY(cudaMalloc(&ix->d_voff[s], slots[s].voff.size() * 4));
-        CUDA_TRY(cudaMemcpy(ix->d_voff[s], slots[s].voff.data(), slots[s].voff.size() * 4, cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMalloc(&ix->d_vals[s], std::max<size_t>(1, slots[s].vals.size()) * 8));
+        CUDA_TRY(ix->d_voff[s].alloc(slots[s].voff.size()));
+        CUDA_TRY(cudaMemcpy(ix->d_voff[s].get(), slots[s].voff.data(), slots[s].voff.size() * 4, cudaMemcpyHostToDevice));
+        CUDA_TRY(ix->d_vals[s].alloc(std::max<size_t>(1, slots[s].vals.size())));
         if (!slots[s].vals.empty())
-            CUDA_TRY(cudaMemcpy(ix->d_vals[s], slots[s].vals.data(), slots[s].vals.size() * 8, cudaMemcpyHostToDevice));
+            CUDA_TRY(cudaMemcpy(ix->d_vals[s].get(), slots[s].vals.data(), slots[s].vals.size() * 8, cudaMemcpyHostToDevice));
         ix->slot_min[s] = slots[s].vals.empty() ? 0 : ~0ull;
         for (uint64_t v : slots[s].vals) { ix->slot_max[s] = std::max(ix->slot_max[s], v); ix->slot_min[s] = std::min(ix->slot_min[s], v); }
         ix->slot_first_min[s] = slots[s].vals.empty() ? 0 : ~0ull;
@@ -551,15 +607,7 @@ extern "C" xgm_status xgm_builder_finish(xgm_builder* b, int device, xgm_index**
     return XGM_OK;
 }
 
-extern "C" void xgm_index_close(xgm_index* ix) {
-    if (!ix) return;
-    cudaSetDevice(ix->device);
-    cudaFree(ix->d_hdr); cudaFree(ix->d_docs); cudaFree(ix->d_tfs); cudaFree(ix->d_doclen);
-    cudaFree(ix->d_bitmaps); cudaFree(ix->d_coarse); cudaFree(ix->d_ranks);
-    for (int s = 0; s < XGM_MAX_SLOTS; ++s) { cudaFree(ix->d_voff[s]); cudaFree(ix->d_vals[s]); }
-    if (ix->compute_stream) cudaStreamDestroy(ix->compute_stream);
-    delete ix;
-}
+extern "C" void xgm_index_close(xgm_index* ix) { delete ix; }
 
 /* ---- synthetic corpus straight into the block format (bench / tests) ---------------------- */
 
@@ -820,9 +868,10 @@ extern "C" xgm_status xgm_term_stats_many(const xgm_index* ix, uint32_t n, const
 
 static void fill_index_params(const xgm_index* ix, XgmKernelParams& p) {
     memset(&p, 0, sizeof(p));
-    p.hdr = ix->d_hdr; p.docs = ix->d_docs; p.tfs = ix->d_tfs; p.doclen = ix->d_doclen; p.lastdocid = ix->lastdocid;
-    p.bitmaps = ix->d_bitmaps; p.coarse = ix->d_coarse; p.ranks = ix->d_ranks; p.doclen_lb = ix->doclen_lb;
-    for (int s = 0; s < XGM_MAX_SLOTS; ++s) { p.slots[s].voff = ix->d_voff[s]; p.slots[s].vals = ix->d_vals[s]; }
+    p.hdr = ix->d_hdr.get(); p.docs = reinterpret_cast<const uint4*>(ix->d_docs.get());
+    p.tfs = reinterpret_cast<const uint4*>(ix->d_tfs.get()); p.doclen = ix->d_doclen.get(); p.lastdocid = ix->lastdocid;
+    p.bitmaps = ix->d_bitmaps.get(); p.coarse = ix->d_coarse.get(); p.ranks = ix->d_ranks.get(); p.doclen_lb = ix->doclen_lb;
+    for (int s = 0; s < XGM_MAX_SLOTS; ++s) { p.slots[s].voff = ix->d_voff[s].get(); p.slots[s].vals = ix->d_vals[s].get(); }
 }
 
 extern "C" xgm_status xgm_index_decode_term(const xgm_index* ix, uint32_t term_id, uint32_t* docids, uint32_t* wdfs,
@@ -834,17 +883,15 @@ extern "C" xgm_status xgm_index_decode_term(const xgm_index* ix, uint32_t term_i
     if (t.termfreq == 0 || (!docids && !wdfs && capacity == 0)) return XGM_OK;
     if (capacity < t.termfreq || !docids || !wdfs) return fail(XGM_E_INVALID, "capacity %u < termfreq %u", capacity, t.termfreq);
     CUDA_TRY(cudaSetDevice(ix->device));
-    uint32_t *dd = nullptr, *dw = nullptr;
+    DevBuf<uint32_t> dd, dw;
     size_t cap = (size_t)t.nblocks * XGM_BLOCK;
-    CUDA_TRY(cudaMalloc(&dd, cap * 4));
-    CUDA_TRY(cudaMalloc(&dw, cap * 4));
+    CUDA_TRY(dd.alloc(cap));
+    CUDA_TRY(dw.alloc(cap));
     XgmKernelParams p;
     fill_index_params(ix, p);
-    cudaError_t e = xgm_launch_decode(p, t.blk_begin, t.nblocks, dd, dw, 0);
-    if (e == cudaSuccess) e = cudaMemcpy(docids, dd, (size_t)t.termfreq * 4, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(wdfs, dw, (size_t)t.termfreq * 4, cudaMemcpyDeviceToHost);
-    cudaFree(dd); cudaFree(dw);
-    if (e != cudaSuccess) return fail(XGM_E_CUDA, "decode: %s", cudaGetErrorString(e));
+    CUDA_TRY(xgm_launch_decode(p, t.blk_begin, t.nblocks, dd.get(), dw.get(), 0));
+    CUDA_TRY(cudaMemcpy(docids, dd.get(), (size_t)t.termfreq * 4, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(wdfs, dw.get(), (size_t)t.termfreq * 4, cudaMemcpyDeviceToHost));
     return XGM_OK;
 }
 
@@ -940,28 +987,19 @@ struct PlannedQuery {
 
 /* A pinned host array and its device copy: the host fills it and one copy uploads it. */
 template <class T> struct PinnedPair {
-    T* h = nullptr;
-    T* d = nullptr;
-    size_t cap = 0;
-    /* room for `need` elements, grown to max(2 need, floor); the stream's copies and kernels may still read the
-     * old buffers, so it is waited for before they are freed */
+    HostBuf<T> h;
+    DevBuf<T> d;
+    cudaError_t alloc(size_t n) {
+        const cudaError_t e = h.alloc(n);
+        return e != cudaSuccess ? e : d.alloc(n);
+    }
     xgm_status reserve(size_t need, size_t floor, cudaStream_t st) {
-        if (need <= cap) return XGM_OK;
-        const size_t c = std::max(need * 2, floor);
-        CUDA_TRY(cudaStreamSynchronize(st));
-        release();
-        CUDA_TRY(cudaMallocHost(&h, c * sizeof(T)));
-        CUDA_TRY(cudaMalloc(&d, c * sizeof(T)));
-        cap = c;
+        CUDA_TRY(h.grow(need, floor, st));
+        CUDA_TRY(d.grow(need, floor, st));
         return XGM_OK;
     }
     cudaError_t upload(size_t n, cudaStream_t st) const {
-        return n ? cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, st) : cudaSuccess;
-    }
-    void release() {
-        if (h) cudaFreeHost(h);
-        cudaFree(d);
-        h = nullptr; d = nullptr; cap = 0;
+        return n ? cudaMemcpyAsync(d.get(), h.get(), n * sizeof(T), cudaMemcpyHostToDevice, st) : cudaSuccess;
     }
 };
 
@@ -970,20 +1008,13 @@ template <class T> struct PinnedPair {
 struct WorkList {
     PinnedPair<XgmWorkItem> seg;  /* segments, in the order the expansion reads them */
     PinnedPair<uint32_t> levels;  /* level starts of a level-ordered expansion */
-    XgmWorkItem* d_exp = nullptr; /* expanded + interleaved work items (device only) */
-    size_t exp_cap = 0;
+    DevBuf<XgmWorkItem> d_exp;    /* expanded + interleaved work items (device only) */
     uint32_t nseg = 0, nstarts = 0, nitems = 0; /* nstarts: entries of `levels` in use */
     /* the segments expand to n work items: room for them on the device */
     xgm_status set_items(uint64_t n, cudaStream_t st) {
         if (n >= 0xffffffffull) return fail(XGM_E_INVALID, "too many work items in one batch");
         nitems = (uint32_t)n;
-        if (n <= exp_cap) return XGM_OK;
-        const size_t c = std::max<size_t>(n * 2, 65536);
-        CUDA_TRY(cudaStreamSynchronize(st));
-        cudaFree(d_exp);
-        d_exp = nullptr; exp_cap = 0;
-        CUDA_TRY(cudaMalloc(&d_exp, c * sizeof(XgmWorkItem)));
-        exp_cap = c;
+        CUDA_TRY(d_exp.grow(n, 65536, st));
         return XGM_OK;
     }
     /* the segments, `extra` rows stored after them, and the level starts */
@@ -991,7 +1022,6 @@ struct WorkList {
         cudaError_t e = seg.upload((size_t)nseg + extra, st);
         return e != cudaSuccess ? e : levels.upload(nstarts, st);
     }
-    void release() { seg.release(); levels.release(); cudaFree(d_exp); }
 };
 
 /* The OR list: one level-ordered expansion per leaf position */
@@ -1005,15 +1035,8 @@ struct OrList : WorkList {
 struct BmList : WorkList {
     bool range_mode = false;
     uint32_t nranges = 1, nruns = 0;
-    uint32_t* d_rng = nullptr; /* per (range, run) first block, item count, output offset */
-    size_t rng_cap = 0;
-    uint32_t* d_rng_total = nullptr; /* [0] = number of items */
-    uint32_t* h_rng_total = nullptr;
-    void release() {
-        WorkList::release();
-        cudaFree(d_rng); cudaFree(d_rng_total);
-        if (h_rng_total) cudaFreeHost(h_rng_total);
-    }
+    DevBuf<uint32_t> d_rng; /* per (range, run) first block, item count, output offset */
+    PinnedPair<uint32_t> rng_total; /* [0] = number of items, counted on the device */
 };
 
 /* A batch's segments as planned, one vector per work list */
@@ -1023,46 +1046,44 @@ struct xgm_searcher {
     const xgm_index* ix = nullptr;
     int device = 0; /* ix->device, kept so that freeing the searcher never reads an index already closed */
     uint32_t max_batch = 0, max_topk = 0, match_cap = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_done = nullptr; /* hand-over between the copy stream and the shared compute stream */
+    Stream stream; /* declared before the buffers and events: destroyed after them */
+    Event ev0, ev1, ev2;
+    Event ev_in, ev_done; /* hand-over between the copy stream and the shared compute stream */
     /* XGM_TRACE=1: one stderr line per batch with its host and GPU timeline (see trace_line) */
-    cudaEvent_t tr_h2d = nullptr, tr_out = nullptr;
+    Event tr_h2d, tr_out;
     std::chrono::steady_clock::time_point tr_submit, tr_planned, tr_launched, tr_async;
     bool shared_compute = true;
     /* pinned host staging */
-    XgmDevQuery* h_queries = nullptr;
-    double* h_out_w = nullptr;
-    uint32_t* h_out_d = nullptr;
-    uint64_t* h_out_k = nullptr;
-    XgmDevResult* h_info = nullptr;
-    XgmRaise* h_raise = nullptr;  /* pinned: raise logs of the batch (copied only when a query asked for them) */
-    XgmRaise* d_raise = nullptr;
-    XgmQState* h_qstate = nullptr; /* pinned: per-query state after the batch (raise-log lengths) */
+    PinnedPair<XgmDevQuery> queries;
+    HostBuf<double> h_out_w;
+    HostBuf<uint32_t> h_out_d;
+    HostBuf<uint64_t> h_out_k;
+    HostBuf<XgmDevResult> h_info;
+    PinnedPair<XgmRaise> raise;  /* raise logs of the batch (copied to the host only when a query asked for them) */
+    HostBuf<XgmQState> h_qstate; /* per-query state after the batch (raise-log lengths) */
     bool any_raise = false;
     uint32_t keep_cap = 0;
     size_t ctrl_bytes = 0;
     /* device */
-    XgmDevQuery* d_queries = nullptr;
     WorkList and_list; /* general AND kernel */
     OrList or_list;
     BmList bm_list;    /* bitmap AND kernel */
     uint32_t bpi = 16;
     uint32_t range_bits = 16; /* XGM_RANGE_BITS: 2^16 docids per range (DESIGN.md §3.1) */
-    uint32_t* d_topk_list = nullptr; /* [max_batch] queries left to the CTA-per-query top-k kernel */
-    unsigned char* d_ctrl = nullptr; /* [XGM_CTRL_HDR B work counters][nq x XgmQState][nq x XGM_NBINS x u32] */
-    double* d_match_w = nullptr;
-    uint32_t* d_match_d = nullptr;
-    uint64_t* d_match_k = nullptr;
-    double* d_pool_w = nullptr;
-    uint32_t* d_pool_d = nullptr;
-    uint64_t* d_pool_k = nullptr;
+    DevBuf<uint32_t> d_topk_list; /* [max_batch] queries left to the CTA-per-query top-k kernel */
+    DevBuf<unsigned char> d_ctrl; /* [XGM_CTRL_HDR B work counters][nq x XgmQState][nq x XGM_NBINS x u32] */
+    DevBuf<double> d_match_w;
+    DevBuf<uint32_t> d_match_d;
+    DevBuf<uint64_t> d_match_k;
+    DevBuf<double> d_pool_w;
+    DevBuf<uint32_t> d_pool_d;
+    DevBuf<uint64_t> d_pool_k;
     uint32_t pool_total = 0;
     double* d_out_w = nullptr;
     uint32_t* d_out_d = nullptr;
     uint64_t* d_out_k = nullptr;
     XgmDevResult* d_info = nullptr;
-    unsigned char* d_slab = nullptr; /* d_out_w | d_out_d | d_info | d_out_k in one allocation: one all-gather moves a shard's MSets */
+    DevBuf<unsigned char> d_slab; /* d_out_w | d_out_d | d_info | d_out_k in one allocation: one all-gather moves a shard's MSets */
     size_t slab_bytes = 0, slab_off_d = 0, slab_off_info = 0, slab_off_k = 0;
     /* last batch */
     std::vector<PlannedQuery> plan;
@@ -1071,8 +1092,7 @@ struct xgm_searcher {
     xgm_batch_stats stats{};
     int grid = 0, grid_or = 0, grid_or3 = 0, grid_tile = 0, grid_bm = 0;
     bool any_or_fast = false, any_or_slow = false;
-    uint32_t* h_tileq = nullptr;  /* pinned: queries of the batch answered by the bitmap-union kernel */
-    uint32_t* d_tileq = nullptr;
+    PinnedPair<uint32_t> tileq;   /* queries of the batch answered by the bitmap-union kernel */
     uint32_t ntileq = 0;
     bool device_only = false;     /* results stay on the device (xgm_searcher_set_results_on_device) */
     uint32_t bpi_override = 0;    /* XGM_BPI: driver blocks per work item for batches >= 256 (default 16) */
@@ -1117,21 +1137,8 @@ extern "C" void xgm_searcher_free(xgm_searcher* s) {
         s->cv.notify_all();
         s->worker.join();
     }
-    cudaSetDevice(s->device);
-    if (s->stream) cudaStreamSynchronize(s->stream);
-    cudaFreeHost(s->h_queries); cudaFreeHost(s->h_out_w); cudaFreeHost(s->h_out_d);
-    cudaFreeHost(s->h_out_k); cudaFreeHost(s->h_info); cudaFreeHost(s->h_raise); cudaFree(s->d_raise); cudaFreeHost(s->h_qstate); cudaFreeHost(s->h_tileq); cudaFree(s->d_tileq);
-    cudaFree(s->d_queries); s->and_list.release(); s->or_list.release(); s->bm_list.release();
-    cudaFree(s->d_ctrl); cudaFree(s->d_topk_list); cudaFree(s->d_match_w); cudaFree(s->d_match_d);
-    cudaFree(s->d_match_k); cudaFree(s->d_pool_w); cudaFree(s->d_pool_d); cudaFree(s->d_pool_k); cudaFree(s->d_slab);
-    if (s->ev0) cudaEventDestroy(s->ev0);
-    if (s->ev1) cudaEventDestroy(s->ev1);
-    if (s->ev2) cudaEventDestroy(s->ev2);
-    if (s->ev_in) cudaEventDestroy(s->ev_in);
-    if (s->tr_h2d) cudaEventDestroy(s->tr_h2d);
-    if (s->tr_out) cudaEventDestroy(s->tr_out);
-    if (s->ev_done) cudaEventDestroy(s->ev_done);
-    if (s->stream) cudaStreamDestroy(s->stream);
+    cudaSetDevice(s->device); /* the members free on the searcher's device */
+    if (s->stream.get()) cudaStreamSynchronize(s->stream.get());
     delete s;
 }
 
@@ -1148,66 +1155,62 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
     s->keep_cap = 2048; /* a power of two (the top-k kernel sorts in place): 2048, 4096 or 8192 */
     while (s->keep_cap < 8192 && s->keep_cap < 8 * max_topk) s->keep_cap <<= 1;
     if (s->keep_cap > s->match_cap) s->keep_cap = s->match_cap;
-    CUDA_TRY(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreate(&s->ev0)); CUDA_TRY(cudaEventCreate(&s->ev1)); CUDA_TRY(cudaEventCreate(&s->ev2));
-    CUDA_TRY(cudaEventCreateWithFlags(&s->ev_in, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&s->ev_done, cudaEventDisableTiming));
+    CUDA_TRY(s->stream.create(cudaStreamNonBlocking));
+    CUDA_TRY(s->ev0.create(cudaEventDefault)); CUDA_TRY(s->ev1.create(cudaEventDefault)); CUDA_TRY(s->ev2.create(cudaEventDefault));
+    CUDA_TRY(s->ev_in.create(cudaEventDisableTiming));
+    CUDA_TRY(s->ev_done.create(cudaEventDisableTiming));
     if (g_trace) {
-        CUDA_TRY(cudaEventCreate(&s->tr_h2d)); CUDA_TRY(cudaEventCreate(&s->tr_out));
+        CUDA_TRY(s->tr_h2d.create(cudaEventDefault)); CUDA_TRY(s->tr_out.create(cudaEventDefault));
         if (!g_tr_base) {
             CUDA_TRY(cudaEventCreate(&g_tr_base));
-            CUDA_TRY(cudaEventRecord(g_tr_base, s->stream));
+            CUDA_TRY(cudaEventRecord(g_tr_base, s->stream.get()));
             CUDA_TRY(cudaEventSynchronize(g_tr_base));
             g_tr_t0 = std::chrono::steady_clock::now();
         }
     }
     if (const char* e = getenv("XGM_SHARED_COMPUTE")) s->shared_compute = atoi(e) != 0;
     if (const char* e = getenv("XGM_RANGE_BITS")) s->range_bits = (uint32_t)std::min(31, std::max(0, atoi(e)));
-    CUDA_TRY(cudaMalloc(&s->bm_list.d_rng_total, 64));
-    CUDA_TRY(cudaMemset(s->bm_list.d_rng_total, 0, 64));
-    CUDA_TRY(cudaMallocHost(&s->bm_list.h_rng_total, 64));
-    s->bm_list.h_rng_total[0] = 0;
+    CUDA_TRY(s->bm_list.rng_total.alloc(16));
+    CUDA_TRY(cudaMemset(s->bm_list.rng_total.d.get(), 0, 64));
+    s->bm_list.rng_total.h.get()[0] = 0;
     {
         std::lock_guard<std::mutex> lk(ix->launch_mu);
-        if (!ix->compute_stream) CUDA_TRY(cudaStreamCreateWithFlags(&ix->compute_stream, cudaStreamNonBlocking));
+        if (!ix->compute_stream.get()) CUDA_TRY(ix->compute_stream.create(cudaStreamNonBlocking));
     }
     size_t nq = max_batch, ns = (size_t)max_batch * max_topk, nm = (size_t)max_batch * s->match_cap;
-    CUDA_TRY(cudaMallocHost(&s->h_queries, nq * sizeof(XgmDevQuery)));
-    CUDA_TRY(cudaMallocHost(&s->h_out_w, ns * 8)); CUDA_TRY(cudaMallocHost(&s->h_out_d, ns * 4));
-    CUDA_TRY(cudaMallocHost(&s->h_out_k, ns * 8)); CUDA_TRY(cudaMallocHost(&s->h_info, nq * sizeof(XgmDevResult)));
-    CUDA_TRY(cudaMalloc(&s->d_queries, nq * sizeof(XgmDevQuery)));
-    CUDA_TRY(cudaMallocHost(&s->h_raise, nq * XGM_RAISE_LOG * sizeof(XgmRaise)));
-    CUDA_TRY(cudaMallocHost(&s->h_qstate, nq * sizeof(XgmQState)));
-    CUDA_TRY(cudaMallocHost(&s->h_tileq, nq * 4));
-    CUDA_TRY(cudaMalloc(&s->d_tileq, nq * 4));
+    CUDA_TRY(s->queries.alloc(nq));
+    CUDA_TRY(s->h_out_w.alloc(ns)); CUDA_TRY(s->h_out_d.alloc(ns));
+    CUDA_TRY(s->h_out_k.alloc(ns)); CUDA_TRY(s->h_info.alloc(nq));
+    CUDA_TRY(s->raise.alloc(nq * XGM_RAISE_LOG));
+    CUDA_TRY(s->h_qstate.alloc(nq));
+    CUDA_TRY(s->tileq.alloc(nq));
     if (const char* e = getenv("XGM_OR_TILE")) s->or_tile = atoi(e) != 0;
     if (const char* e = getenv("XGM_OR_KERNEL")) s->or_general = atoi(e) == 1;
     if (const char* e = getenv("XGM_BPI")) s->bpi_override = (uint32_t)std::min(32, std::max(0, atoi(e)));
-    CUDA_TRY(cudaMalloc(&s->d_raise, nq * XGM_RAISE_LOG * sizeof(XgmRaise)));
     s->ctrl_bytes = XGM_CTRL_HDR + nq * sizeof(XgmQState) + nq * XGM_NBINS * 4;
-    CUDA_TRY(cudaMalloc(&s->d_ctrl, s->ctrl_bytes));
-    CUDA_TRY(cudaMalloc(&s->d_topk_list, (size_t)nq * 4));
-    CUDA_TRY(cudaMalloc(&s->d_match_w, nm * 8)); CUDA_TRY(cudaMalloc(&s->d_match_d, nm * 4)); CUDA_TRY(cudaMalloc(&s->d_match_k, nm * 8));
+    CUDA_TRY(s->d_ctrl.alloc(s->ctrl_bytes));
+    CUDA_TRY(s->d_topk_list.alloc(nq));
+    CUDA_TRY(s->d_match_w.alloc(nm)); CUDA_TRY(s->d_match_d.alloc(nm)); CUDA_TRY(s->d_match_k.alloc(nm));
     {
         auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
         s->slab_off_d = up(ns * 8);
         s->slab_off_info = s->slab_off_d + up(ns * 4);
         s->slab_off_k = s->slab_off_info + up(nq * sizeof(XgmDevResult));
         s->slab_bytes = s->slab_off_k + up(ns * 8);
-        CUDA_TRY(cudaMalloc(&s->d_slab, s->slab_bytes));
-        s->d_out_w = reinterpret_cast<double*>(s->d_slab);
-        s->d_out_d = reinterpret_cast<uint32_t*>(s->d_slab + s->slab_off_d);
-        s->d_info = reinterpret_cast<XgmDevResult*>(s->d_slab + s->slab_off_info);
-        s->d_out_k = reinterpret_cast<uint64_t*>(s->d_slab + s->slab_off_k);
+        CUDA_TRY(s->d_slab.alloc(s->slab_bytes));
+        s->d_out_w = reinterpret_cast<double*>(s->d_slab.get());
+        s->d_out_d = reinterpret_cast<uint32_t*>(s->d_slab.get() + s->slab_off_d);
+        s->d_info = reinterpret_cast<XgmDevResult*>(s->d_slab.get() + s->slab_off_info);
+        s->d_out_k = reinterpret_cast<uint64_t*>(s->d_slab.get() + s->slab_off_k);
     }
     /* overflow pool: room for the tie mass of a few pathological queries per batch (doccount entries at least) */
     s->pool_total = std::max<uint32_t>(1u << 20, std::min<uint32_t>(1u << 25, 2 * ix->doccount + (1u << 16)));
     if (const char* e = getenv("XGM_POOL_ENTRIES")) s->pool_total = (uint32_t)strtoul(e, nullptr, 10);
-    CUDA_TRY(cudaMalloc(&s->d_pool_w, (size_t)s->pool_total * 8)); CUDA_TRY(cudaMalloc(&s->d_pool_d, (size_t)s->pool_total * 4));
-    CUDA_TRY(cudaMalloc(&s->d_pool_k, (size_t)s->pool_total * 8));
-    xgm_status st = s->and_list.seg.reserve(4096, 4096, s->stream);
-    if (st == XGM_OK) st = s->or_list.seg.reserve(4096, 4096, s->stream);
-    if (st == XGM_OK) st = s->bm_list.seg.reserve(4096, 4096, s->stream);
+    CUDA_TRY(s->d_pool_w.alloc(s->pool_total)); CUDA_TRY(s->d_pool_d.alloc(s->pool_total));
+    CUDA_TRY(s->d_pool_k.alloc(s->pool_total));
+    xgm_status st = s->and_list.seg.reserve(4096, 4096, s->stream.get());
+    if (st == XGM_OK) st = s->or_list.seg.reserve(4096, 4096, s->stream.get());
+    if (st == XGM_OK) st = s->bm_list.seg.reserve(4096, 4096, s->stream.get());
     if (st != XGM_OK) return st;
     int occ = xgm_and_occupancy_blocks_per_sm();
     if (occ < 1) occ = 1;
@@ -1228,7 +1231,7 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
     return XGM_OK;
 }
 
-extern "C" void* xgm_searcher_stream(xgm_searcher* s) { return s ? (void*)s->stream : nullptr; }
+extern "C" void* xgm_searcher_stream(xgm_searcher* s) { return s ? (void*)s->stream.get() : nullptr; }
 
 /* ComparePostListTermFreqAscending on (tf, original index) — same std::partial_sort_copy call as
  * MultiAndPostList's constructor (multiandpostlist.h:126-131) so ties land identically (libstdc++). */
@@ -1397,8 +1400,8 @@ static xgm_status resolve_terms(const xgm_index* ix, const xgm_query& q, PlanTer
     if (q.sort_by > XGM_SORT_REL_VAL || q.filter > XGM_FILTER_MULTI_RANGE) return XGM_E_INVALID;
     if ((q.filter && q.filter_slot >= XGM_MAX_SLOTS) || (q.sort_by && q.sort_slot >= XGM_MAX_SLOTS)) return XGM_E_INVALID;
     if (q.revision != 0 && q.revision != ix->revision) return XGM_E_STALE;
-    if ((q.filter && !ix->slot_exact[q.filter_slot] && ix->d_voff[q.filter_slot]) ||
-        (q.sort_by && !ix->slot_exact[q.sort_slot] && ix->d_voff[q.sort_slot]))
+    if ((q.filter && !ix->slot_exact[q.filter_slot] && ix->d_voff[q.filter_slot].get()) ||
+        (q.sort_by && !ix->slot_exact[q.sort_slot] && ix->d_voff[q.sort_slot].get()))
         return XGM_E_UNIMPLEMENTED; /* values longer than 8 bytes: their keys do not decide the comparison */
     /* a weighted range source: a child of the AND (or of a single term) without groups, with a factor >= 0 */
     if (q.filter_weighted && (q.filter != XGM_FILTER_MULTI_RANGE || (q.op != XGM_OP_AND && q.nterms != 1) || groups ||
@@ -1769,9 +1772,9 @@ static xgm_status order_levels(WorkList& L, std::vector<XgmWorkItem>& v, uint32_
         const uint32_t maxlev = (v[0].b0 + bpi - 1) / bpi;
         r = L.levels.reserve((size_t)maxlev + 1, 1024, st);
         if (r != XGM_OK) return r;
-        run = level_starts(v.data(), v.size(), maxlev, bpi, L.levels.h);
+        run = level_starts(v.data(), v.size(), maxlev, bpi, L.levels.h.get());
         L.nstarts = maxlev + 1;
-        std::copy(v.begin(), v.end(), L.seg.h);
+        std::copy(v.begin(), v.end(), L.seg.h.get());
     }
     L.nseg = (uint32_t)v.size();
     return L.set_items(run, st);
@@ -1804,14 +1807,14 @@ static xgm_status order_or_groups(OrList& L, std::vector<XgmWorkItem>& v, uint32
         g.seg_off = (uint32_t)a; g.level_off = (uint32_t)lvpos;
         g.nlevels = (v[a].b0 + bpi - 1) / bpi;
         g.out_off = (uint32_t)run;
-        const uint64_t n = level_starts(v.data() + a, b - a, g.nlevels, bpi, L.levels.h + lvpos);
+        const uint64_t n = level_starts(v.data() + a, b - a, g.nlevels, bpi, L.levels.h.get() + lvpos);
         g.total = (uint32_t)n;
         run += n;
         lvpos += (size_t)g.nlevels + 1;
         L.groups.push_back(g);
         a = b;
     }
-    std::copy(v.begin(), v.end(), L.seg.h);
+    std::copy(v.begin(), v.end(), L.seg.h.get());
     L.nseg = (uint32_t)v.size();
     L.nstarts = (uint32_t)lvpos;
     return L.set_items(run, st);
@@ -1825,15 +1828,15 @@ static xgm_status order_or_groups(OrList& L, std::vector<XgmWorkItem>& v, uint32
  * number of items: every range can add one partial item per run. */
 static xgm_status order_driver_runs(xgm_searcher* s, std::vector<XgmWorkItem>& v, uint32_t bpi) {
     BmList& L = s->bm_list;
-    xgm_status r = L.seg.reserve(2 * v.size(), 4096, s->stream); /* segments, then at most as many runs */
+    xgm_status r = L.seg.reserve(2 * v.size(), 4096, s->stream.get()); /* segments, then at most as many runs */
     if (r != XGM_OK) return r;
     L.nranges = (s->ix->lastdocid >> s->range_bits) + 1;
-    const XgmDevQuery* hq = s->h_queries;
+    const XgmDevQuery* hq = s->queries.h.get();
     auto drv = [hq](const XgmWorkItem& a) { return hq[a.query].terms[0].blk_begin; };
     std::sort(v.begin(), v.end(), [&](const XgmWorkItem& a, const XgmWorkItem& b) {
         return drv(a) != drv(b) ? drv(a) < drv(b) : a.query < b.query;
     });
-    XgmWorkItem* h = L.seg.h;
+    XgmWorkItem* h = L.seg.h.get();
     const size_t nseg = v.size();
     uint64_t run = 0;
     for (size_t i = 0; i < nseg; ++i) {
@@ -1852,29 +1855,22 @@ static xgm_status order_driver_runs(xgm_searcher* s, std::vector<XgmWorkItem>& v
     });
     run += (uint64_t)L.nruns * L.nranges;
     const size_t need = (size_t)L.nranges * L.nruns * 3; /* first blocks, counts, offsets */
-    if (need > L.rng_cap) {
-        CUDA_TRY(cudaStreamSynchronize(s->stream));
-        if (s->ix->compute_stream) CUDA_TRY(cudaStreamSynchronize(s->ix->compute_stream));
-        cudaFree(L.d_rng);
-        L.d_rng = nullptr; L.rng_cap = 0;
-        CUDA_TRY(cudaMalloc(&L.d_rng, need * 2 * sizeof(uint32_t)));
-        L.rng_cap = need * 2;
-    }
+    CUDA_TRY(L.d_rng.grow(need, 0, s->stream.get()));
     L.nseg = (uint32_t)nseg;
     L.nstarts = 0;
-    return L.set_items(run, s->stream);
+    return L.set_items(run, s->stream.get());
 }
 
 static cudaError_t expand_levels(const WorkList& L, uint32_t bpi, cudaStream_t cs, uint32_t& launches) {
     if (!L.nitems) return cudaSuccess;
     ++launches;
-    return xgm_launch_expand(L.seg.d, L.nitems, L.levels.d, L.nstarts - 1, bpi, L.d_exp, cs);
+    return xgm_launch_expand(L.seg.d.get(), L.nitems, L.levels.d.get(), L.nstarts - 1, bpi, L.d_exp.get(), cs);
 }
 
 static cudaError_t expand_or_groups(const OrList& L, uint32_t bpi, cudaStream_t cs, uint32_t& launches) {
     for (const auto& g : L.groups) {
-        cudaError_t e = xgm_launch_expand(L.seg.d + g.seg_off, g.total, L.levels.d + g.level_off, g.nlevels, bpi,
-                                          L.d_exp + g.out_off, cs);
+        cudaError_t e = xgm_launch_expand(L.seg.d.get() + g.seg_off, g.total, L.levels.d.get() + g.level_off, g.nlevels,
+                                          bpi, L.d_exp.get() + g.out_off, cs);
         if (e != cudaSuccess) return e;
         ++launches;
     }
@@ -1885,8 +1881,8 @@ static cudaError_t expand_driver_runs(const BmList& L, const XgmBlockHdr* hdr, u
                                       cudaStream_t cs, uint32_t& launches) {
     const size_t n = (size_t)L.nranges * L.nruns;
     launches += 3;
-    return xgm_launch_expand_ranges(L.seg.d + L.nseg, L.nruns, hdr, L.nranges, range_bits, bpi, L.d_rng, L.d_rng + n,
-                                    L.d_rng + 2 * n, L.d_rng_total, L.d_exp, cs);
+    return xgm_launch_expand_ranges(L.seg.d.get() + L.nseg, L.nruns, hdr, L.nranges, range_bits, bpi, L.d_rng.get(),
+                                    L.d_rng.get() + n, L.d_rng.get() + 2 * n, L.rng_total.d.get(), L.d_exp.get(), cs);
 }
 
 /* The match kernels of one pass (p.pass) over the batch's work lists */
@@ -1909,14 +1905,14 @@ static xgm_status launch_batch(xgm_searcher* s) {
     /* batches that fill the GPU on their own run their kernels on the index's FIFO compute stream; small
      * ones (concurrent single queries of many host threads) stay on the searcher's stream and share the SMs */
     const bool shared = s->shared_compute && s->nq >= 256;
-    cudaStream_t cs = shared ? s->ix->compute_stream : s->stream;
+    cudaStream_t cs = shared ? s->ix->compute_stream.get() : s->stream.get();
     std::unique_lock<std::mutex> lk(s->ix->launch_mu, std::defer_lock);
     if (shared) {
-        CUDA_TRY(cudaEventRecord(s->ev_in, s->stream));
+        CUDA_TRY(cudaEventRecord(s->ev_in.get(), s->stream.get()));
         lk.lock(); /* one batch's launches stay contiguous in the shared stream */
-        CUDA_TRY(cudaStreamWaitEvent(cs, s->ev_in, 0));
+        CUDA_TRY(cudaStreamWaitEvent(cs, s->ev_in.get(), 0));
     }
-    CUDA_TRY(cudaMemsetAsync(s->d_ctrl, 0, XGM_CTRL_HDR + (size_t)s->max_batch * sizeof(XgmQState), cs));
+    CUDA_TRY(cudaMemsetAsync(s->d_ctrl.get(), 0, XGM_CTRL_HDR + (size_t)s->max_batch * sizeof(XgmQState), cs));
     CUDA_TRY(cudaMemsetAsync(p.hist, 0, (size_t)s->nq * XGM_NBINS * 4, cs));
     s->stats.kernel_launches = 0;
     p.pass = 0;
@@ -1925,10 +1921,10 @@ static xgm_status launch_batch(xgm_searcher* s) {
     CUDA_TRY(expand_or_groups(s->or_list, s->bpi, cs, launches));
     CUDA_TRY(s->bm_list.range_mode ? expand_driver_runs(s->bm_list, p.hdr, s->range_bits, s->bpi, cs, launches)
                                    : expand_levels(s->bm_list, s->bpi, cs, launches));
-    CUDA_TRY(cudaEventRecord(s->ev0, cs));
+    CUDA_TRY(cudaEventRecord(s->ev0.get(), cs));
     xgm_status st = launch_match(s, p, cs);
     if (st != XGM_OK) return st;
-    CUDA_TRY(cudaEventRecord(s->ev1, cs));
+    CUDA_TRY(cudaEventRecord(s->ev1.get(), cs));
     CUDA_TRY(xgm_launch_topk(p, s->nq, cs));
     s->stats.kernel_launches += (s->nq >= 64 && p.topk_list) ? 2 : 1; /* xgm_topk_small_kernel + xgm_topk_kernel */
     /* second pass: only queries whose candidate buffer overflowed do any work (device-side flag) */
@@ -1938,11 +1934,11 @@ static xgm_status launch_batch(xgm_searcher* s) {
     if (st != XGM_OK) return st;
     CUDA_TRY(xgm_launch_topk(p2, s->nq, cs));
     s->stats.kernel_launches++;
-    CUDA_TRY(cudaEventRecord(s->ev2, cs));
+    CUDA_TRY(cudaEventRecord(s->ev2.get(), cs));
     if (shared) {
-        CUDA_TRY(cudaEventRecord(s->ev_done, cs));
+        CUDA_TRY(cudaEventRecord(s->ev_done.get(), cs));
         lk.unlock();
-        CUDA_TRY(cudaStreamWaitEvent(s->stream, s->ev_done, 0));
+        CUDA_TRY(cudaStreamWaitEvent(s->stream.get(), s->ev_done.get(), 0));
     }
     return XGM_OK;
 }
@@ -1950,6 +1946,8 @@ static xgm_status launch_batch(xgm_searcher* s) {
 static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_t nq) {
     const auto t_submit0 = std::chrono::steady_clock::now();
     CUDA_TRY(cudaSetDevice(s->ix->device));
+    const cudaStream_t stream = s->stream.get();
+    XgmDevQuery* const hq = s->queries.h.get();
     s->plan.resize(nq);
     s->nq = nq;
     PlannedSegments segs;
@@ -1965,13 +1963,13 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     int T = 1;
     if (nq >= 512) T = PlannerPool::get().threads();
     if (T <= 1) {
-        for (uint32_t i = 0; i < nq; ++i) plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], segs);
+        for (uint32_t i = 0; i < nq; ++i) plan_query(s, queries[i], i, s->plan[i], hq[i], segs);
     } else {
         std::vector<PlannedSegments> ts(T);
         PlannerPool::get().run(T, [&](int t) {
             uint32_t a = (uint32_t)((uint64_t)nq * t / T), b = (uint32_t)((uint64_t)nq * (t + 1) / T);
             ts[t].bm_list.reserve((size_t)(b - a));
-            for (uint32_t i = a; i < b; ++i) plan_query(s, queries[i], i, s->plan[i], s->h_queries[i], ts[t]);
+            for (uint32_t i = a; i < b; ++i) plan_query(s, queries[i], i, s->plan[i], hq[i], ts[t]);
         });
         for (int t = 0; t < T; ++t) {
             segs.and_list.insert(segs.and_list.end(), ts[t].and_list.begin(), ts[t].and_list.end());
@@ -1981,7 +1979,7 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     }
     const auto t_planned = std::chrono::steady_clock::now();
     for (uint32_t i = 0; i < nq; ++i) {
-        if (s->plan[i].sort_by || s->h_queries[i].route == XGM_ROUTE_OR || s->plan[i].aux_subqs) s->any_sort = true; /* keys/aux needed on the host */
+        if (s->plan[i].sort_by || hq[i].route == XGM_ROUTE_OR || s->plan[i].aux_subqs) s->any_sort = true; /* keys/aux needed on the host */
         alg += s->plan[i].alg_bytes;
     }
     /* segments → each list's pinned staging, in the order the device expands them */
@@ -1989,9 +1987,9 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     BmList& bm = s->bm_list;
     bm.range_mode = !segs.bm_list.empty() && nq >= 256 && s->range_bits != 0;
     bm.nruns = 0;
-    xgm_status st = order_levels(s->and_list, segs.and_list, bpi, s->stream);
-    if (st == XGM_OK) st = order_or_groups(s->or_list, segs.or_list, bpi, s->stream);
-    if (st == XGM_OK) st = bm.range_mode ? order_driver_runs(s, segs.bm_list, bpi) : order_levels(bm, segs.bm_list, bpi, s->stream);
+    xgm_status st = order_levels(s->and_list, segs.and_list, bpi, stream);
+    if (st == XGM_OK) st = order_or_groups(s->or_list, segs.or_list, bpi, stream);
+    if (st == XGM_OK) st = bm.range_mode ? order_driver_runs(s, segs.bm_list, bpi) : order_levels(bm, segs.bm_list, bpi, stream);
     if (st != XGM_OK) return st;
     const auto t_interleaved = std::chrono::steady_clock::now();
     s->stats = xgm_batch_stats{};
@@ -2001,37 +1999,37 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
     s->stats.d2h_bytes = (uint64_t)nq * sizeof(XgmDevResult) + (uint64_t)nq * s->max_topk * (8 + 4 + (s->any_sort ? 8 : 0));
     XgmKernelParams& p = s->params;
     fill_index_params(s->ix, p);
-    p.queries = s->d_queries; p.items = s->and_list.d_exp; p.nitems = s->and_list.nitems; p.nq = nq;
-    p.items_or = s->or_list.d_exp; p.nitems_or = s->or_list.nitems;
-    p.items_bm = bm.d_exp; p.nitems_bm = bm.nitems;
-    p.nitems_bm_dev = bm.range_mode ? bm.d_rng_total : nullptr;
-    p.bm_segs = bm.range_mode ? bm.seg.d : nullptr;
-    p.work_counter = reinterpret_cast<uint32_t*>(s->d_ctrl);
-    p.qstate = reinterpret_cast<XgmQState*>(s->d_ctrl + XGM_CTRL_HDR);
-    p.hist = reinterpret_cast<uint32_t*>(s->d_ctrl + XGM_CTRL_HDR + (size_t)s->max_batch * sizeof(XgmQState));
-    p.topk_list = s->d_topk_list;
+    p.queries = s->queries.d.get(); p.items = s->and_list.d_exp.get(); p.nitems = s->and_list.nitems; p.nq = nq;
+    p.items_or = s->or_list.d_exp.get(); p.nitems_or = s->or_list.nitems;
+    p.items_bm = bm.d_exp.get(); p.nitems_bm = bm.nitems;
+    p.nitems_bm_dev = bm.range_mode ? bm.rng_total.d.get() : nullptr;
+    p.bm_segs = bm.range_mode ? bm.seg.d.get() : nullptr;
+    p.work_counter = reinterpret_cast<uint32_t*>(s->d_ctrl.get());
+    p.qstate = reinterpret_cast<XgmQState*>(s->d_ctrl.get() + XGM_CTRL_HDR);
+    p.hist = reinterpret_cast<uint32_t*>(s->d_ctrl.get() + XGM_CTRL_HDR + (size_t)s->max_batch * sizeof(XgmQState));
+    p.topk_list = s->d_topk_list.get();
     p.match_cap = s->match_cap; p.keep_cap = s->keep_cap;
-    p.pool_total = s->pool_total; p.pool_w = s->d_pool_w; p.pool_d = s->d_pool_d; p.pool_k = s->d_pool_k;
-    p.match_w = s->d_match_w; p.match_d = s->d_match_d; p.match_k = s->d_match_k;
+    p.pool_total = s->pool_total; p.pool_w = s->d_pool_w.get(); p.pool_d = s->d_pool_d.get(); p.pool_k = s->d_pool_k.get();
+    p.match_w = s->d_match_w.get(); p.match_d = s->d_match_d.get(); p.match_k = s->d_match_k.get();
     p.out_stride = s->max_topk; p.out_w = s->d_out_w; p.out_d = s->d_out_d; p.out_k = s->d_out_k; p.out_info = s->d_info;
-    p.raise_log = s->d_raise;
+    p.raise_log = s->raise.d.get();
     s->any_raise = false;
     for (uint32_t i = 0; i < nq; ++i) s->any_raise |= s->plan[i].log_raises;
     s->any_or_fast = s->any_or_slow = false;
     s->ntileq = 0;
     for (uint32_t i = 0; i < nq; ++i)
-        if (s->h_queries[i].route == XGM_ROUTE_OR && s->plan[i].on_device) {
-            if (s->h_queries[i].or_fast == XGM_OR_FAST_TILE) s->h_tileq[s->ntileq++] = i;
-            else if (s->h_queries[i].or_fast == XGM_OR_FAST_OR3) s->any_or_fast = true;
+        if (hq[i].route == XGM_ROUTE_OR && s->plan[i].on_device) {
+            if (hq[i].or_fast == XGM_OR_FAST_TILE) s->tileq.h.get()[s->ntileq++] = i;
+            else if (hq[i].or_fast == XGM_OR_FAST_OR3) s->any_or_fast = true;
             else s->any_or_slow = true;
         }
-    p.tileq = s->d_tileq; p.ntileq = s->ntileq;
-    if (s->ntileq) CUDA_TRY(cudaMemcpyAsync(s->d_tileq, s->h_tileq, (size_t)s->ntileq * 4, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(s->d_queries, s->h_queries, (size_t)nq * sizeof(XgmDevQuery), cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(s->and_list.upload(0, s->stream));
-    CUDA_TRY(s->or_list.upload(0, s->stream));
-    CUDA_TRY(bm.upload(bm.nruns, s->stream)); /* the runs follow the segments */
-    if (g_trace) { s->tr_submit = t_submit0; s->tr_planned = t_interleaved; CUDA_TRY(cudaEventRecord(s->tr_h2d, s->stream)); }
+    p.tileq = s->tileq.d.get(); p.ntileq = s->ntileq;
+    CUDA_TRY(s->tileq.upload(s->ntileq, stream));
+    CUDA_TRY(s->queries.upload(nq, stream));
+    CUDA_TRY(s->and_list.upload(0, stream));
+    CUDA_TRY(s->or_list.upload(0, stream));
+    CUDA_TRY(bm.upload(bm.nruns, stream)); /* the runs follow the segments */
+    if (g_trace) { s->tr_submit = t_submit0; s->tr_planned = t_interleaved; CUDA_TRY(cudaEventRecord(s->tr_h2d.get(), stream)); }
     st = launch_batch(s);
     if (st != XGM_OK) return st;
     size_t ns = (size_t)nq * s->max_topk;
@@ -2041,18 +2039,18 @@ static xgm_status submit_impl(xgm_searcher* s, const xgm_query* queries, uint32_
         s->stats.host_plan_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_submit0).count();
         return XGM_OK;
     }
-    CUDA_TRY(cudaMemcpyAsync(s->h_info, s->d_info, (size_t)nq * sizeof(XgmDevResult), cudaMemcpyDeviceToHost, s->stream));
-    if (bm.range_mode) CUDA_TRY(cudaMemcpyAsync(bm.h_rng_total, bm.d_rng_total, 4, cudaMemcpyDeviceToHost, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(s->h_out_w, s->d_out_w, ns * 8, cudaMemcpyDeviceToHost, s->stream));
-    CUDA_TRY(cudaMemcpyAsync(s->h_out_d, s->d_out_d, ns * 4, cudaMemcpyDeviceToHost, s->stream));
-    if (s->any_sort) CUDA_TRY(cudaMemcpyAsync(s->h_out_k, s->d_out_k, ns * 8, cudaMemcpyDeviceToHost, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(s->h_info.get(), s->d_info, (size_t)nq * sizeof(XgmDevResult), cudaMemcpyDeviceToHost, stream));
+    if (bm.range_mode) CUDA_TRY(cudaMemcpyAsync(bm.rng_total.h.get(), bm.rng_total.d.get(), 4, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(s->h_out_w.get(), s->d_out_w, ns * 8, cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(s->h_out_d.get(), s->d_out_d, ns * 4, cudaMemcpyDeviceToHost, stream));
+    if (s->any_sort) CUDA_TRY(cudaMemcpyAsync(s->h_out_k.get(), s->d_out_k, ns * 8, cudaMemcpyDeviceToHost, stream));
     if (s->any_raise) {
-        CUDA_TRY(cudaMemcpyAsync(s->h_raise, s->d_raise, (size_t)nq * XGM_RAISE_LOG * sizeof(XgmRaise), cudaMemcpyDeviceToHost, s->stream));
-        CUDA_TRY(cudaMemcpyAsync(s->h_qstate, s->d_ctrl + XGM_CTRL_HDR, (size_t)nq * sizeof(XgmQState), cudaMemcpyDeviceToHost, s->stream));
+        CUDA_TRY(cudaMemcpyAsync(s->raise.h.get(), s->raise.d.get(), (size_t)nq * XGM_RAISE_LOG * sizeof(XgmRaise), cudaMemcpyDeviceToHost, stream));
+        CUDA_TRY(cudaMemcpyAsync(s->h_qstate.get(), s->d_ctrl.get() + XGM_CTRL_HDR, (size_t)nq * sizeof(XgmQState), cudaMemcpyDeviceToHost, stream));
     }
     s->pending = true;
     s->stats.host_plan_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_submit0).count();
-    if (g_trace) { CUDA_TRY(cudaEventRecord(s->tr_out, s->stream)); s->tr_launched = std::chrono::steady_clock::now(); }
+    if (g_trace) { CUDA_TRY(cudaEventRecord(s->tr_out.get(), stream)); s->tr_launched = std::chrono::steady_clock::now(); }
     if (getenv("XGM_DEBUG_TIMING"))
         fprintf(stderr, "xgm submit: plan %.3f ms, interleave %.3f ms, enqueue %.3f ms (T=%d, items %zu)\n",
                 std::chrono::duration<float, std::milli>(t_planned - t_submit0).count(),
@@ -2199,11 +2197,11 @@ static void trace_line(xgm_searcher* s, std::chrono::steady_clock::time_point wa
                        std::chrono::steady_clock::time_point joined, std::chrono::steady_clock::time_point synced) {
     auto ms = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double, std::milli>(t - g_tr_t0).count(); };
     float g[5] = {0, 0, 0, 0, 0};
-    cudaEventElapsedTime(&g[0], g_tr_base, s->tr_h2d);
-    cudaEventElapsedTime(&g[1], g_tr_base, s->ev0);
-    cudaEventElapsedTime(&g[2], g_tr_base, s->ev1);
-    cudaEventElapsedTime(&g[3], g_tr_base, s->ev2);
-    cudaEventElapsedTime(&g[4], g_tr_base, s->tr_out);
+    cudaEventElapsedTime(&g[0], g_tr_base, s->tr_h2d.get());
+    cudaEventElapsedTime(&g[1], g_tr_base, s->ev0.get());
+    cudaEventElapsedTime(&g[2], g_tr_base, s->ev1.get());
+    cudaEventElapsedTime(&g[3], g_tr_base, s->ev2.get());
+    cudaEventElapsedTime(&g[4], g_tr_base, s->tr_out.get());
     fprintf(stderr, "XGMTRACE s=%p nq=%u host async=%.3f start=%.3f planned=%.3f enq=%.3f wait=%.3f joined=%.3f synced=%.3f done=%.3f "
             "gpu h2d=%.3f k0=%.3f k1=%.3f k2=%.3f out=%.3f second_pass=%u\n", (void*)s, s->nq, ms(s->tr_async), ms(s->tr_submit), ms(s->tr_planned),
             ms(s->tr_launched), ms(wait_in), ms(joined), ms(synced), ms(std::chrono::steady_clock::now()), g[0], g[1], g[2], g[3], g[4], s->stats.second_pass_queries);
@@ -2220,29 +2218,30 @@ extern "C" xgm_status xgm_search_wait(xgm_searcher* s, uint32_t* docids, double*
     }
     const auto tr_joined = std::chrono::steady_clock::now();
     CUDA_TRY(cudaSetDevice(s->ix->device));
-    cudaError_t e = cudaStreamSynchronize(s->stream);
+    cudaError_t e = cudaStreamSynchronize(s->stream.get());
     s->pending = false;
     if (e != cudaSuccess) return fail(XGM_E_CUDA, "batch failed: %s", cudaGetErrorString(e));
     if (s->device_only) return XGM_OK; /* nothing was copied: the results are in the device slab */
-    cudaEventElapsedTime(&s->stats.match_kernel_ms, s->ev0, s->ev1);
-    cudaEventElapsedTime(&s->stats.topk_kernel_ms, s->ev1, s->ev2);
+    cudaEventElapsedTime(&s->stats.match_kernel_ms, s->ev0.get(), s->ev1.get());
+    cudaEventElapsedTime(&s->stats.topk_kernel_ms, s->ev1.get(), s->ev2.get());
     const auto t_wait0 = std::chrono::steady_clock::now();
-    if (s->bm_list.range_mode) s->stats.work_items = (uint64_t)s->and_list.nitems + s->or_list.nitems + s->bm_list.h_rng_total[0];
+    if (s->bm_list.range_mode) s->stats.work_items = (uint64_t)s->and_list.nitems + s->or_list.nitems + s->bm_list.rng_total.h.get()[0];
     s->stats.second_pass_queries = 0;
     for (uint32_t i = 0; i < s->nq; ++i) {
         const PlannedQuery& pq = s->plan[i];
         const size_t off = (size_t)i * s->max_topk;
-        if (pq.status == XGM_OK && pq.on_device && (s->h_info[i].flags & XGM_RES_SECOND_PASS)) s->stats.second_pass_queries++;
-        finish_info(pq, &s->h_info[i], s->any_sort ? s->h_out_k + off : nullptr,
-                    s->h_queries[i].route == XGM_ROUTE_OR || pq.aux_subqs, &info[i],
-                    s->any_raise ? s->h_raise + (size_t)i * XGM_RAISE_LOG : nullptr, s->any_raise ? s->h_qstate[i].nraise : 0u);
-        if (pq.status == XGM_OK && pq.on_device) s->stats.algorithmic_bytes += 4ull * s->h_info[i].exact;
+        const XgmDevResult& dr = s->h_info.get()[i];
+        if (pq.status == XGM_OK && pq.on_device && (dr.flags & XGM_RES_SECOND_PASS)) s->stats.second_pass_queries++;
+        finish_info(pq, &dr, s->any_sort ? s->h_out_k.get() + off : nullptr,
+                    s->queries.h.get()[i].route == XGM_ROUTE_OR || pq.aux_subqs, &info[i],
+                    s->any_raise ? s->raise.h.get() + (size_t)i * XGM_RAISE_LOG : nullptr, s->any_raise ? s->h_qstate.get()[i].nraise : 0u);
+        if (pq.status == XGM_OK && pq.on_device) s->stats.algorithmic_bytes += 4ull * dr.exact;
         uint32_t n = info[i].n;
         if (n > stride) return fail(XGM_E_INVALID, "stride %u too small for %u results", stride, n);
         if (n && docids && weights) {
-            memcpy(docids + (size_t)i * stride, s->h_out_d + off + pq.first, (size_t)n * 4);
-            memcpy(weights + (size_t)i * stride, s->h_out_w + off + pq.first, (size_t)n * 8);
-            if (sort_keys && pq.sort_by) memcpy(sort_keys + (size_t)i * stride, s->h_out_k + off + pq.first, (size_t)n * 8);
+            memcpy(docids + (size_t)i * stride, s->h_out_d.get() + off + pq.first, (size_t)n * 4);
+            memcpy(weights + (size_t)i * stride, s->h_out_w.get() + off + pq.first, (size_t)n * 8);
+            if (sort_keys && pq.sort_by) memcpy(sort_keys + (size_t)i * stride, s->h_out_k.get() + off + pq.first, (size_t)n * 8);
         }
     }
     s->stats.host_wait_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_wait0).count();
@@ -2281,7 +2280,7 @@ extern "C" xgm_status xgm_search_device_results(xgm_searcher* s, void** weights,
 extern "C" xgm_status xgm_search_device_slab(xgm_searcher* s, void** base, uint64_t* bytes, uint64_t* off_docids,
                                              uint64_t* off_counts, uint32_t* stride) {
     if (!s) return fail(XGM_E_INVALID, "null argument");
-    if (base) *base = s->d_slab;
+    if (base) *base = s->d_slab.get();
     if (bytes) *bytes = s->slab_bytes;
     if (off_docids) *off_docids = s->slab_off_d;
     if (off_counts) *off_counts = s->slab_off_info;
@@ -2298,9 +2297,9 @@ extern "C" xgm_status xgm_search_device_slab_keys(xgm_searcher* s, uint64_t* off
 extern "C" xgm_status xgm_search_last_stats(xgm_searcher* s, xgm_batch_stats* out) {
     if (!s || !out) return fail(XGM_E_INVALID, "null argument");
     if (!s->pending && s->nq) {
-        cudaEventSynchronize(s->ev2);
-        cudaEventElapsedTime(&s->stats.match_kernel_ms, s->ev0, s->ev1);
-        cudaEventElapsedTime(&s->stats.topk_kernel_ms, s->ev1, s->ev2);
+        cudaEventSynchronize(s->ev2.get());
+        cudaEventElapsedTime(&s->stats.match_kernel_ms, s->ev0.get(), s->ev1.get());
+        cudaEventElapsedTime(&s->stats.topk_kernel_ms, s->ev1.get(), s->ev2.get());
     }
     *out = s->stats;
     return XGM_OK;
@@ -2310,7 +2309,7 @@ extern "C" xgm_status xgm_index_copy_doclengths(const xgm_index* ix, uint32_t fi
     if (!ix || (n && !out)) return fail(XGM_E_INVALID, "null argument");
     if ((uint64_t)first_docid + n > (uint64_t)ix->lastdocid + 1) return fail(XGM_E_INVALID, "docid range beyond lastdocid");
     CUDA_TRY(cudaSetDevice(ix->device));
-    if (n) CUDA_TRY(cudaMemcpy(out, ix->d_doclen + first_docid, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    if (n) CUDA_TRY(cudaMemcpy(out, ix->d_doclen.get() + first_docid, (size_t)n * 4, cudaMemcpyDeviceToHost));
     return XGM_OK;
 }
 
