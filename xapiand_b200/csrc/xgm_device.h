@@ -100,24 +100,34 @@ struct XgmKernelParams {
 #define XGM_CTRL_HDR 128 /* bytes of work counters in front of the per-query state */
 static_assert(4 * (XGM_WC_TOPK_BACK + 1) <= XGM_CTRL_HDR, "the work counters fit their header");
 
+/* Largest keep_cap of a searcher: the top-k kernel holds XGM_KEEP_PER_THREAD survivors per thread in registers. */
+#define XGM_KEEP_CAP_MAX 8192u
+
+/* Resident-CTA grids of the persistent kernels for one searcher. */
+struct XgmGrids {
+    int and_, and_bm, or_, or3, or_tile, topk;
+};
+/* The grids on the current device at sm_count SMs, the top-k kernel's at keep_cap.  Also opts the kernels with large
+ * dynamic shared memory in on the current device, each at a constant size: the bitmap AND and or3 kernels at their
+ * fixed scratch, the top-k kernel at XGM_KEEP_CAP_MAX.  Searchers of any keep_cap, created on any thread, write the
+ * same values. */
+cudaError_t xgm_kernel_grids(int sm_count, uint32_t keep_cap, XgmGrids& g);
+
 cudaError_t xgm_launch_and(const XgmKernelParams& p, int grid, cudaStream_t s);
 cudaError_t xgm_launch_and_bm(const XgmKernelParams& p, int grid, cudaStream_t s);
-int xgm_and_bm_occupancy_blocks_per_sm();
 cudaError_t xgm_launch_expand(const XgmWorkItem* seg, uint32_t total, const uint32_t* level_start, uint32_t nlevels,
                               uint32_t bpi, XgmWorkItem* out, cudaStream_t s);
 cudaError_t xgm_launch_expand_ranges(const XgmWorkItem* runs, uint32_t nruns, const XgmBlockHdr* hdr, uint32_t nranges,
                                      uint32_t range_bits, uint32_t bpi, uint32_t* lo, uint32_t* cnt, uint32_t* off,
                                      uint32_t* total, XgmWorkItem* out, cudaStream_t s);
 cudaError_t xgm_launch_or(const XgmKernelParams& p, int grid, cudaStream_t s);
-int xgm_or_occupancy_blocks_per_sm();
 cudaError_t xgm_launch_or3(const XgmKernelParams& p, int grid, int phase, cudaStream_t s);
 cudaError_t xgm_launch_or_tile(const XgmKernelParams& p, int grid, cudaStream_t s);
-int xgm_or_tile_occupancy_blocks_per_sm();
-int xgm_or3_occupancy_blocks_per_sm();
-cudaError_t xgm_launch_topk(const XgmKernelParams& p, uint32_t nq, cudaStream_t s);
+/* Ranks the batch's nq queries on at most `grid` CTAs; adds the kernels it enqueued (one or two) to `launches`. */
+cudaError_t xgm_launch_topk(const XgmKernelParams& p, uint32_t nq, int grid, uint32_t& launches, cudaStream_t s);
 cudaError_t xgm_launch_coarse(const uint32_t* bitmaps, size_t ncoarse, uint32_t* coarse, cudaStream_t s);
-cudaError_t xgm_launch_decode(const XgmKernelParams& p, uint32_t blk_begin, uint32_t nblocks, uint32_t* out_d,
-                              uint32_t* out_w, cudaStream_t s);
+cudaError_t xgm_launch_decode(const XgmKernelParams& p, uint32_t blk_begin, uint32_t nblocks, int sm_count,
+                              uint32_t* out_d, uint32_t* out_w, cudaStream_t s);
 size_t xgm_topk_smem_bytes(uint32_t keep_cap);
 /* xgm_merge_kernel's inputs: nparts gathered parts, part p of each array at base + p * part_* bytes, [query][rank]
  * records of `stride` per query; outputs [nq][maxitems] records and [nq] counts. */
@@ -134,7 +144,13 @@ struct XgmMergeArgs {
     uint64_t* out_k;
     uint32_t* out_n;
 };
+#define XGM_MERGE_MAX_PARTS 64
+#define XGM_MERGE_MAX_SMEM (200 * 1024) /* bytes of dynamic shared memory a merge may take */
+/* xgm_merge_kernel's dynamic shared memory: weight, docid and, when keys are read, key of m records per part */
+static inline uint64_t xgm_merge_smem_bytes(uint32_t nparts, uint64_t m, bool keys) {
+    return nparts * m * (keys ? 20 : 12);
+}
+/* The caller checks nparts and xgm_merge_smem_bytes against the limits above. */
 cudaError_t xgm_launch_merge(const XgmMergeArgs& a, cudaStream_t s);
-int xgm_and_occupancy_blocks_per_sm();
 
 #endif

@@ -889,7 +889,7 @@ extern "C" xgm_status xgm_index_decode_term(const xgm_index* ix, uint32_t term_i
     CUDA_TRY(dw.alloc(cap));
     XgmKernelParams p;
     fill_index_params(ix, p);
-    CUDA_TRY(xgm_launch_decode(p, t.blk_begin, t.nblocks, dd.get(), dw.get(), 0));
+    CUDA_TRY(xgm_launch_decode(p, t.blk_begin, t.nblocks, ix->sm_count, dd.get(), dw.get(), 0));
     CUDA_TRY(cudaMemcpy(docids, dd.get(), (size_t)t.termfreq * 4, cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(wdfs, dw.get(), (size_t)t.termfreq * 4, cudaMemcpyDeviceToHost));
     return XGM_OK;
@@ -1090,7 +1090,7 @@ struct xgm_searcher {
     uint32_t nq = 0;
     bool pending = false, any_sort = false;
     xgm_batch_stats stats{};
-    int grid = 0, grid_or = 0, grid_or3 = 0, grid_tile = 0, grid_bm = 0;
+    XgmGrids grids{};
     bool any_or_fast = false, any_or_slow = false;
     PinnedPair<uint32_t> tileq;   /* queries of the batch answered by the bitmap-union kernel */
     uint32_t ntileq = 0;
@@ -1151,10 +1151,9 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
     s->ix = ix; s->device = ix->device; s->max_batch = max_batch; s->max_topk = max_topk;
     /* candidates a query may buffer before its pruning threshold settles (~k(1+ln(M/k)) arrive above
      * a rising threshold) and how many of them the top-k kernel can hold in shared memory */
-    s->match_cap = std::min<uint32_t>(65536, std::max<uint32_t>(8192, 32 * max_topk));
-    s->keep_cap = 2048; /* a power of two (the top-k kernel sorts in place): 2048, 4096 or 8192 */
-    while (s->keep_cap < 8192 && s->keep_cap < 8 * max_topk) s->keep_cap <<= 1;
-    if (s->keep_cap > s->match_cap) s->keep_cap = s->match_cap;
+    s->match_cap = std::min<uint32_t>(65536, std::max<uint32_t>(XGM_KEEP_CAP_MAX, 32 * max_topk));
+    s->keep_cap = 2048; /* a power of two (the top-k kernel sorts in place): 2048, 4096 or XGM_KEEP_CAP_MAX */
+    while (s->keep_cap < XGM_KEEP_CAP_MAX && s->keep_cap < 8 * max_topk) s->keep_cap <<= 1;
     CUDA_TRY(s->stream.create(cudaStreamNonBlocking));
     CUDA_TRY(s->ev0.create(cudaEventDefault)); CUDA_TRY(s->ev1.create(cudaEventDefault)); CUDA_TRY(s->ev2.create(cudaEventDefault));
     CUDA_TRY(s->ev_in.create(cudaEventDisableTiming));
@@ -1212,21 +1211,7 @@ extern "C" xgm_status xgm_searcher_new(const xgm_index* ix, uint32_t max_batch, 
     if (st == XGM_OK) st = s->or_list.seg.reserve(4096, 4096, s->stream.get());
     if (st == XGM_OK) st = s->bm_list.seg.reserve(4096, 4096, s->stream.get());
     if (st != XGM_OK) return st;
-    int occ = xgm_and_occupancy_blocks_per_sm();
-    if (occ < 1) occ = 1;
-    s->grid = ix->sm_count * occ;
-    occ = xgm_or_occupancy_blocks_per_sm();
-    if (occ < 1) occ = 1;
-    s->grid_or = ix->sm_count * occ;
-    occ = xgm_or3_occupancy_blocks_per_sm();
-    if (occ < 1) occ = 1;
-    s->grid_or3 = ix->sm_count * occ;
-    occ = xgm_or_tile_occupancy_blocks_per_sm();
-    if (occ < 1) occ = 1;
-    s->grid_tile = ix->sm_count * occ;
-    occ = xgm_and_bm_occupancy_blocks_per_sm();
-    if (occ < 1) occ = 1;
-    s->grid_bm = ix->sm_count * occ;
+    CUDA_TRY(xgm_kernel_grids(ix->sm_count, s->keep_cap, s->grids));
     *out = s.release();
     return XGM_OK;
 }
@@ -1888,13 +1873,14 @@ static cudaError_t expand_driver_runs(const BmList& L, const XgmBlockHdr* hdr, u
 /* The match kernels of one pass (p.pass) over the batch's work lists */
 static xgm_status launch_match(xgm_searcher* s, const XgmKernelParams& p, cudaStream_t cs) {
     uint32_t& launches = s->stats.kernel_launches;
-    if (s->bm_list.nitems) { CUDA_TRY(xgm_launch_and_bm(p, s->grid_bm, cs)); ++launches; }
-    if (s->and_list.nitems) { CUDA_TRY(xgm_launch_and(p, s->grid, cs)); ++launches; }
-    if (s->or_list.nitems && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p, s->grid_or3, 0, cs)); ++launches; }
-    if (s->or_list.nitems && s->any_or_slow) { CUDA_TRY(xgm_launch_or(p, s->grid_or, cs)); ++launches; }
+    const XgmGrids& g = s->grids;
+    if (s->bm_list.nitems) { CUDA_TRY(xgm_launch_and_bm(p, g.and_bm, cs)); ++launches; }
+    if (s->and_list.nitems) { CUDA_TRY(xgm_launch_and(p, g.and_, cs)); ++launches; }
+    if (s->or_list.nitems && s->any_or_fast) { CUDA_TRY(xgm_launch_or3(p, g.or3, 0, cs)); ++launches; }
+    if (s->or_list.nitems && s->any_or_slow) { CUDA_TRY(xgm_launch_or(p, g.or_, cs)); ++launches; }
     if (s->ntileq) { /* documents with >= 2 leaves by bitmap union, then the single-leaf ones against the threshold */
-        CUDA_TRY(xgm_launch_or_tile(p, s->grid_tile, cs));
-        CUDA_TRY(xgm_launch_or3(p, s->grid_or3, 1, cs));
+        CUDA_TRY(xgm_launch_or_tile(p, g.or_tile, cs));
+        CUDA_TRY(xgm_launch_or3(p, g.or3, 1, cs));
         launches += 2;
     }
     return XGM_OK;
@@ -1925,15 +1911,13 @@ static xgm_status launch_batch(xgm_searcher* s) {
     xgm_status st = launch_match(s, p, cs);
     if (st != XGM_OK) return st;
     CUDA_TRY(cudaEventRecord(s->ev1.get(), cs));
-    CUDA_TRY(xgm_launch_topk(p, s->nq, cs));
-    s->stats.kernel_launches += (s->nq >= 64 && p.topk_list) ? 2 : 1; /* xgm_topk_small_kernel + xgm_topk_kernel */
+    CUDA_TRY(xgm_launch_topk(p, s->nq, s->grids.topk, launches, cs));
     /* second pass: only queries whose candidate buffer overflowed do any work (device-side flag) */
     XgmKernelParams p2 = p;
     p2.pass = 1;
     st = launch_match(s, p2, cs);
     if (st != XGM_OK) return st;
-    CUDA_TRY(xgm_launch_topk(p2, s->nq, cs));
-    s->stats.kernel_launches++;
+    CUDA_TRY(xgm_launch_topk(p2, s->nq, s->grids.topk, launches, cs));
     CUDA_TRY(cudaEventRecord(s->ev2.get(), cs));
     if (shared) {
         CUDA_TRY(cudaEventRecord(s->ev_done.get(), cs));
@@ -2397,7 +2381,8 @@ extern "C" xgm_status xgm_merge_topk_device(const void* gw, const void* gd, cons
                                             void* cuda_stream) {
     if (!gw || !gd || !ginfo || !out_w || !out_d || !out_n || nparts == 0 || nq == 0 || k == 0 || k > stride)
         return fail(XGM_E_INVALID, "bad arguments");
-    if ((size_t)nparts * k * 12 > 200 * 1024 || nparts > 64) return fail(XGM_E_INVALID, "nparts*k too large for the merge kernel");
+    if (xgm_merge_smem_bytes(nparts, k, false) > XGM_MERGE_MAX_SMEM || nparts > XGM_MERGE_MAX_PARTS)
+        return fail(XGM_E_INVALID, "nparts*k too large for the merge kernel");
     XgmMergeArgs a = rel_merge_args(nparts, nq, stride, k, out_w, out_d, out_n);
     a.gw = static_cast<const double*>(gw); a.gd = static_cast<const uint32_t*>(gd);
     a.ginfo = static_cast<const XgmDevResult*>(ginfo);
@@ -2425,7 +2410,8 @@ extern "C" xgm_status xgm_merge_topk_device_slab(const void* gathered, uint64_t 
         return fail(XGM_E_INVALID, "bad arguments");
     xgm_status st = check_slab_layout(slab_bytes, off_docids, off_counts, 0, false, nq, stride);
     if (st != XGM_OK) return st;
-    if ((size_t)nparts * k * 12 > 200 * 1024 || nparts > 64) return fail(XGM_E_INVALID, "nparts*k too large for the merge kernel");
+    if (xgm_merge_smem_bytes(nparts, k, false) > XGM_MERGE_MAX_SMEM || nparts > XGM_MERGE_MAX_PARTS)
+        return fail(XGM_E_INVALID, "nparts*k too large for the merge kernel");
     const unsigned char* g = static_cast<const unsigned char*>(gathered);
     XgmMergeArgs a = rel_merge_args(nparts, nq, stride, k, out_w, out_d, out_n);
     a.gw = reinterpret_cast<const double*>(g); a.gd = reinterpret_cast<const uint32_t*>(g + off_docids);
@@ -2445,7 +2431,8 @@ extern "C" xgm_status xgm_merge_mset_device_slab(const void* gathered, uint64_t 
         return fail(XGM_E_INVALID, "bad arguments");
     xgm_status st = check_slab_layout(slab_bytes, off_docids, off_counts, off_keys, true, nq, stride);
     if (st != XGM_OK) return st;
-    if ((uint64_t)nparts * (first + maxitems) * 20 > 200 * 1024 || nparts > 64)
+    /* the limit counts the keys whether or not the orders read them */
+    if (xgm_merge_smem_bytes(nparts, (uint64_t)first + maxitems, true) > XGM_MERGE_MAX_SMEM || nparts > XGM_MERGE_MAX_PARTS)
         return fail(XGM_E_INVALID, "nparts*(first+maxitems) too large for the merge kernel");
     const unsigned char* g = static_cast<const unsigned char*>(gathered);
     XgmMergeArgs a{};

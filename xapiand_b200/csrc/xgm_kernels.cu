@@ -28,21 +28,6 @@
 
 #define FULL 0xffffffffu
 
-/* cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device attribute and one process may drive several
- * GPUs through the C-ABI (an xgm_index carries its device): remember the opted-in size per (kernel, device). */
-#define XGM_MAX_DEVICES 64
-static cudaError_t optin_smem(const void* fn, int which, size_t bytes) {
-    static size_t have[2][XGM_MAX_DEVICES]; /* raised monotonically; racing threads set the same or a larger value */
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    if (dev < 0 || dev >= XGM_MAX_DEVICES) return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (bytes <= have[which][dev]) return cudaSuccess;
-    e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e == cudaSuccess) have[which][dev] = bytes;
-    return e;
-}
-
 /* ------------------------------------------------------------------ PTX helpers */
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -1102,16 +1087,6 @@ cudaError_t xgm_launch_and_bm(const XgmKernelParams& p, int grid, cudaStream_t s
     return cudaGetLastError();
 }
 
-/* Also opts the kernel in to its dynamic shared memory on the CURRENT device (the attribute is per device:
- * call once per searcher, after cudaSetDevice). */
-int xgm_and_bm_occupancy_blocks_per_sm() {
-    int n = 0;
-    const size_t smem = sizeof(Bm3Scratch) * BM3_WARPS;
-    cudaFuncSetAttribute(xgm_and_bm3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_and_bm3_kernel, BM3_WARPS * 32, smem);
-    return n;
-}
-
 /* ------------------------------------------------------------------ OR kernel */
 
 #define OR_WARPS 4
@@ -1507,16 +1482,6 @@ cudaError_t xgm_launch_or3(const XgmKernelParams& p, int grid, int phase, cudaSt
     return cudaGetLastError();
 }
 
-/* also opts in to the dynamic shared memory on the current device (call once per searcher) */
-int xgm_or3_occupancy_blocks_per_sm() {
-    int n = 0;
-    const size_t smem = sizeof(Or3Scratch) * OR3_WARPS;
-    cudaFuncSetAttribute(xgm_or3_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(xgm_or3_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_or3_kernel<0>, OR3_WARPS * 32, smem);
-    return n;
-}
-
 /* ------------------------------------------------------------------ OR by bitmap union (documents with >= 2 leaves) */
 
 /* For an OR whose leaves all have membership bitmaps the union needs no posting list at all: word w of the
@@ -1641,12 +1606,6 @@ cudaError_t xgm_launch_or_tile(const XgmKernelParams& p, int grid, cudaStream_t 
     return cudaGetLastError();
 }
 
-int xgm_or_tile_occupancy_blocks_per_sm() {
-    int n = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_or_tile_kernel, TILE_WARPS * 32, 0);
-    return n;
-}
-
 /* ------------------------------------------------------------------ top-k / ProtoMSet */
 
 /* Strict total order of the reference's comparators (msetcmp.cc:54-98) with ascending docid order:
@@ -1669,7 +1628,8 @@ __device__ __forceinline__ bool ranks_before(uint32_t sort_by, uint32_t reverse,
 
 #define TOPK_THREADS 256
 #define XGM_EXACT_COUNT_MAX 1024u /* largest match set whose ProtoMSet count is reproduced exactly */
-#define XGM_KEEP_PER_THREAD 32   /* keep_cap <= 8192 = 32 * TOPK_THREADS */
+#define XGM_KEEP_PER_THREAD 32
+static_assert(XGM_KEEP_CAP_MAX == XGM_KEEP_PER_THREAD * TOPK_THREADS, "every survivor of a full keep_cap has a register");
 
 /* Sort key of a match as up to five 32-bit words, most significant first, such that a larger key ranks
  * earlier under the reference's comparators (msetcmp.cc:54-98, ascending docid order):
@@ -2319,7 +2279,6 @@ __global__ void __launch_bounds__(TOPK_THREADS) xgm_topk_kernel(XgmKernelParams 
  * is LOST or PENDING holds no answer for the query, and an order byte above 7 names no order, so such a query
  * gets count UINT32_MAX and no records rather than a merge that silently misses that shard's documents.  The
  * order is the same for the whole CTA, so its branches do not diverge. */
-#define XGM_MERGE_MAX_PARTS 64
 /* 8 CTAs per SM: 32 registers, the full 2048 threads wherever shared memory allows it (no spills) */
 __global__ void __launch_bounds__(256, 8) xgm_merge_kernel(const XgmMergeArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -2389,10 +2348,9 @@ __global__ void __launch_bounds__(256, 8) xgm_merge_kernel(const XgmMergeArgs a)
 }
 
 cudaError_t xgm_launch_merge(const XgmMergeArgs& a, cudaStream_t s) {
-    if (a.nparts > XGM_MERGE_MAX_PARTS) return cudaErrorInvalidValue;
-    const size_t smem = (size_t)a.nparts * (a.first + a.maxitems) * (a.gk ? 20 : 12);
-    if (smem > 48 * 1024) {
-        cudaError_t e = optin_smem((const void*)xgm_merge_kernel, 0, smem);
+    const size_t smem = xgm_merge_smem_bytes(a.nparts, a.first + a.maxitems, a.gk != nullptr);
+    if (smem > 48 * 1024) { /* at the constant limit: concurrent merges of any size opt in to the same value */
+        cudaError_t e = cudaFuncSetAttribute(xgm_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XGM_MERGE_MAX_SMEM);
         if (e != cudaSuccess) return e;
     }
     xgm_merge_kernel<<<a.nq, 256, smem, s>>>(a);
@@ -2626,53 +2584,51 @@ cudaError_t xgm_launch_or(const XgmKernelParams& p, int grid, cudaStream_t s) {
 
 size_t xgm_topk_smem_bytes(uint32_t keep_cap) { return (size_t)keep_cap * (8 + 8 + 4) + XGM_NBINS * 4; }
 
-cudaError_t xgm_launch_topk(const XgmKernelParams& p, uint32_t nq, cudaStream_t s) {
-    size_t smem = xgm_topk_smem_bytes(p.keep_cap);
-    if (smem > 48 * 1024) {
-        cudaError_t e = optin_smem((const void*)xgm_topk_kernel, 1, smem);
-        if (e != cudaSuccess) return e;
-    }
+cudaError_t xgm_launch_topk(const XgmKernelParams& p, uint32_t nq, int grid, uint32_t& launches, cudaStream_t s) {
     XgmKernelParams pp = p;
     pp.nq = nq;
     /* first pass of a real batch: the few-match queries are ranked a warp each, the rest listed for the CTAs */
-    if (p.pass == 0 && nq >= 64 && p.topk_list != nullptr)
+    if (p.pass == 0 && nq >= 64 && p.topk_list != nullptr) {
         xgm_topk_small_kernel<<<(nq + TOPK_SMALL_WARPS - 1) / TOPK_SMALL_WARPS, TOPK_SMALL_WARPS * 32, 0, s>>>(pp);
-    else
+        ++launches;
+    } else {
         pp.topk_list = nullptr;
-    static int ctas = 0; /* resident CTAs of the persistent kernel on this device class */
-    if (ctas == 0) {
-        int dev = 0, sms = 0, occ = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, xgm_topk_kernel, TOPK_THREADS, smem);
-        ctas = sms * (occ > 0 ? occ : 1);
     }
-    const uint32_t grid = nq < (uint32_t)ctas ? nq : (uint32_t)ctas;
-    xgm_topk_kernel<<<grid, TOPK_THREADS, smem, s>>>(pp);
+    xgm_topk_kernel<<<nq < (uint32_t)grid ? nq : (uint32_t)grid, TOPK_THREADS, xgm_topk_smem_bytes(p.keep_cap), s>>>(pp);
+    ++launches;
     return cudaGetLastError();
 }
 
-cudaError_t xgm_launch_decode(const XgmKernelParams& p, uint32_t blk_begin, uint32_t nblocks, uint32_t* out_d,
-                              uint32_t* out_w, cudaStream_t s) {
+cudaError_t xgm_launch_decode(const XgmKernelParams& p, uint32_t blk_begin, uint32_t nblocks, int sm_count,
+                              uint32_t* out_d, uint32_t* out_w, cudaStream_t s) {
     int grid = (int)((nblocks + MATCH_WARPS - 1) / MATCH_WARPS);
-    int dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms < 1) sms = 132; /* H100 SXM */
-    if (grid > sms * 8) grid = sms * 8;
+    if (grid > sm_count * 8) grid = sm_count * 8;
     if (grid < 1) grid = 1;
     xgm_decode_kernel<<<grid, MATCH_WARPS * 32, 0, s>>>(p, blk_begin, nblocks, out_d, out_w);
     return cudaGetLastError();
 }
 
-int xgm_and_occupancy_blocks_per_sm() {
-    int n = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_and_kernel, MATCH_WARPS * 32, 0);
-    return n;
-}
-
-int xgm_or_occupancy_blocks_per_sm() {
-    int n = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, xgm_or_kernel, OR_WARPS * 32, 0);
-    return n;
+cudaError_t xgm_kernel_grids(int sm_count, uint32_t keep_cap, XgmGrids& g) {
+    cudaError_t e = cudaSuccess;
+    auto check = [&e](cudaError_t r) { if (e == cudaSuccess) e = r; };
+    auto optin = [&](const void* fn, size_t bytes) {
+        check(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    };
+    auto resident = [&](const void* fn, int threads, size_t smem) {
+        int occ = 0;
+        check(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, threads, smem));
+        return sm_count * (occ > 0 ? occ : 1);
+    };
+    const size_t bm_smem = sizeof(Bm3Scratch) * BM3_WARPS, or3_smem = sizeof(Or3Scratch) * OR3_WARPS;
+    optin((const void*)xgm_and_bm3_kernel, bm_smem);
+    optin((const void*)xgm_or3_kernel<0>, or3_smem);
+    optin((const void*)xgm_or3_kernel<1>, or3_smem);
+    optin((const void*)xgm_topk_kernel, xgm_topk_smem_bytes(XGM_KEEP_CAP_MAX));
+    g.and_ = resident((const void*)xgm_and_kernel, MATCH_WARPS * 32, 0);
+    g.and_bm = resident((const void*)xgm_and_bm3_kernel, BM3_WARPS * 32, bm_smem);
+    g.or_ = resident((const void*)xgm_or_kernel, OR_WARPS * 32, 0);
+    g.or3 = resident((const void*)xgm_or3_kernel<0>, OR3_WARPS * 32, or3_smem);
+    g.or_tile = resident((const void*)xgm_or_tile_kernel, TILE_WARPS * 32, 0);
+    g.topk = resident((const void*)xgm_topk_kernel, TOPK_THREADS, xgm_topk_smem_bytes(keep_cap));
+    return e;
 }
